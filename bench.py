@@ -2,19 +2,22 @@
 """Benchmark of the SM3Det sparse-MoE backbone hot path (BASELINE.json metric: backbone images/s @1024^2, bs = 32).
 
   python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference]
-                  [--config t_e8|b_e16|lsk_s] [--global-batch G | --batch B] [--expert-parallel]
+                  [--config t_e8|b_e16|lsk_s] [--global-batch G | --batch B] [--expert-parallel] [--dump-outputs DIR]
 
 One "step" = forward + backward of the backbone over the GLOBAL batch of synthetic 1024^2 tiles:
   t_e8  (default) BASELINE configs[1]/[2]: ConvNeXt-T, E = 8 top-2, MoE in the last two stages every other block.
         Global batch 32 at every N (the batch the metric is quoted on) -> strong scaling: 32 / 16 / 8 / 4 images per GPU at
-        N = 1 / 2 / 4 / 8, each GPU's share in ONE forward/backward pass (61 GB of activations at 32 images; `--micro-batch 8`
-        splits it with gradient accumulation, measured 4 % slower; `--global-batch 8` is configs[1] literally).  N > 1: one
+        N = 1 / 2 / 4 / 8, each GPU's share in forward/backward passes of at most 16 images with gradient accumulation (one
+        32-image pass holds 61 GB of activations, and its CUDA graph does not fit next to them in 80 GB; `--micro-batch 32`
+        runs it eagerly; `--global-batch 8` is configs[1] literally).  N > 1: one
         process per GPU (torchrun), one flat gradient all-reduce per step over NCCL, captured in the step's CUDA graph
         (`--cuda-graph off` = eager launches under DistributedDataParallel).  Gating is the reference constructor's default
         (noisy top-k while training); `--noisy-gating off` = deterministic routing.
   b_e16 BASELINE configs[3]: ConvNeXt-B, E = 16, all 36 blocks MoE; experts sharded over the ranks when N > 1.
   lsk_s BASELINE configs[4]: LSKNet-S MoE, SyncBN, global batch 16 (4 GPUs -> 4 per GPU).
-The timed region is bracketed by barrier + synchronize and the max over ranks is reported.  `--impl reference` times the
+The timed region is bracketed by barrier + synchronize and the max over ranks is reported.  `--dump-outputs DIR` writes what
+the last timed step computed (pyramid features over all its micro-batches, the gate loss of each micro-batch, the step
+value, the parameter gradients) as DIR/<name>.npy, so that two builds can be compared on identical inputs.  `--impl reference` times the
 reference's own CPU implementation of the same path (the oracle port: identical torch CPU ops in the reference's order)
 on the box's host cores.
 """
@@ -36,7 +39,7 @@ sys.path.insert(0, ROOT)
 METRIC = 'backbone images/sec @1024^2 (fwd+bwd)'
 NOISY_DEFAULT = 'config'
 CONFIGS = {
-    't_e8': dict(family='convnext', global_batch=32, micro=32,
+    't_e8': dict(family='convnext', global_batch=32, micro=16,
                  kw=dict(arch='tiny', MoE_Block_inds=[[], [], [0, 2, 4, 6, 8], [0, 2]], num_experts=8, top_k=2,
                          noisy_gating=True, drop_path_rate=0.0),
                  name='SM3Det ConvNeXt-T e8t2 last-2-blocks MoE backbone (BASELINE configs[1]/[2])'),
@@ -70,6 +73,10 @@ def parse():
                     help='N > 1: shard the experts over the ranks (NVLink peer-memory dispatch); default for --config b_e16')
     ap.add_argument('--no-expert-parallel', action='store_true')
     ap.add_argument('--cpu-images', type=int, default=1, help='images in the bounded CPU sample')
+    ap.add_argument('--dump-outputs', default=None, metavar='DIR',
+                    help='write the last timed step\'s outputs as DIR/<name>.npy: out0..out3 over all micro-batches, gate_loss per '
+                         'micro-batch, step_value, grad_sample (all parameter gradients); float32, arrays above 2^21 '
+                         'elements as a fixed seeded sample')
     ap.add_argument('--noisy-gating', choices=['config', 'off'], default=NOISY_DEFAULT,
                     help="ConvNeXt configs: 'config' = the reference constructor's default (noisy top-k gating while training, "
                          "what configs/SM3Det/*.py run), 'off' = deterministic routing")
@@ -182,8 +189,8 @@ def oracle_step(fwd, sd, x):
 def time_cpu_reference(args, images, steps, warmup):
     """fwd+bwd (the bench metric) and eval forward (what north_star names as the CPU baseline) of the oracle port."""
     from sm3det_b200.synth import make_images
-    # torch's CPU kernels stop scaling (and then collapse: 143 s/img at 128 threads vs 1.5 s at 16 on the 128-thread
-    # B200 host, profiles/r01_cpu_threads.txt) long before the box runs out of cores: use the best-performing count.
+    # torch's CPU kernels stop scaling (and then collapse at 128 threads) long before a large host runs out of cores:
+    # use at most 16 threads.
     threads = int(os.environ.get('SM3_CPU_THREADS', min(16, os.cpu_count() or 1)))
     torch.set_num_threads(threads)
     fwd, sd = oracle_model(args.config)
@@ -206,15 +213,15 @@ def cpu_baseline_entry(args, ips, dt, threads, fwd_ips):
     return {'value': ips, 'unit': 'img/s', 'cores': threads, 'kind': 'port', 'host_cpus': os.cpu_count(),
             'eval_forward_img_s': fwd_ips,
             'sample': f'fwd+bwd of {args.cpu_images} workload image(s) per step (oracle port = the reference\'s torch CPU fp32 '
-                      f'ops in its order), {threads} of {os.cpu_count()} host threads (torch CPU stops scaling beyond, '
-                      f'profiles/r01_cpu_threads.txt), {dt:.1f} s/step; eval_forward_img_s = one eval forward of the same images'}
+                      f'ops in its order), {threads} of {os.cpu_count()} host threads (torch CPU stops scaling beyond), '
+                      f'{dt:.1f} s/step; eval_forward_img_s = one eval forward of the same images'}
 
 
 def run_reference(args):
     rank = int(os.environ.get('RANK', '0'))
     if rank != 0:
         return
-    steps, warmup = max(1, min(args.steps, 3)), min(args.warmup, 1)
+    steps, warmup = max(1, args.steps), args.warmup
     ips, dt, threads, fwd_ips = time_cpu_reference(args, args.cpu_images, steps, warmup)
     _, _, _, scaling, _ = resolve(args, args.gpus)
     line = {'impl': 'reference', 'metric': METRIC, 'value': ips, 'unit': 'img/s', 'n_gpus': args.gpus, 'steps': steps,
@@ -227,7 +234,7 @@ def run_reference(args):
 
 def time_gpu_eager(args, micro):
     """The GPU-side comparator (SURVEY 8d, BASELINE.md 3): the reference's own module graph -- here its oracle port, the same
-    torch ops -- run in eager PyTorch on this B200 (cuBLAS / cuDNN / ATen kernels), fp32 and with TF32 allowed, timed with
+    torch ops -- run in eager PyTorch on the same GPU (cuBLAS / cuDNN / ATen kernels), fp32 and with TF32 allowed, timed with
     CUDA events like tools/analysis_tools/benchmark.py:118-146.  Not the product: the number our kernels have to beat."""
     from sm3det_b200.synth import make_images
     fwd, sd = oracle_model(args.config)
@@ -258,7 +265,10 @@ def time_gpu_eager(args, micro):
 
 
 # ------------------------------------------------------------------------------------------------
-TENSOR_OPS = ('gemm', 'ffn_fused_fwd', 'ffn_fused_bwd')     # ops.* entry points that launch tcgen05 kernels
+TENSOR_OPS = ('gemm', 'ffn_fused_fwd', 'ffn_fused_bwd')     # ops.* entry points that launch wgmma kernels
+# Roofline denominators when MEASURED_PEAKS.json (measured on the card) is absent: NVIDIA's H100 SXM data sheet, dense bf16
+# and HBM3 at a 700 W power limit.  A card set to a lower power limit reaches less; the line says which source was used.
+H100_BF16_TFLOPS, H100_HBM_GBS = 989.0, 3350.0
 
 
 def gemm_roofline(step_fn, peaks):
@@ -300,15 +310,17 @@ def gemm_roofline(step_fn, peaks):
                 ms = a.elapsed_time(b)
                 f.write(f'{name} shape={shape} ms={ms:.4f} tflops={fl / ms * 1e-9:.1f}\n')
     tot_flops = sum(r[2] for r in rec)
-    peak = peaks.get('bf16_tflops_sustained') or peaks.get('bf16_tflops') or 1590.0
+    measured = peaks.get('bf16_tflops_sustained') or peaks.get('bf16_tflops')
+    peak = measured or H100_BF16_TFLOPS
     ach = tot_flops / (tot_ms * 1e-3) / 1e12 if tot_ms > 0 else 0.0
-    return {'bound': 'tensor', 'kernel': 'tcgen05 kernels (gemm_bf16x3 + fused FFN), all launches of one fwd+bwd micro-batch',
+    return {'bound': 'tensor', 'kernel': 'wgmma kernels (gemm_bf16x3 + fused FFN), all launches of one fwd+bwd micro-batch',
             'achieved': ach, 'peak': peak, 'unit': 'TFLOP/s', 'frac': ach / peak, 'traffic': None, 'launches': len(rec),
+            'peak_source': 'measured cuBLAS bf16 (sustained), MEASURED_PEAKS.json' if measured
+                           else 'H100 SXM data sheet, dense bf16 at 700 W (not measured on this card)',
             'algorithmic_bytes_per_launch': sum(r[3] for r in rec) / max(len(rec), 1),
             'tensor_ms_per_micro_batch': tot_ms, 'algorithmic_tflop_per_micro_batch': tot_flops / 1e12,
             'note': 'algorithmic fp32 FLOPs; each costs 3 bf16 tensor-core MACs (hi*hi+hi*lo+lo*hi), so the tensor pipe '
-                    'runs at 3x this rate (ceiling of frac = 1/3); peak = measured cuBLAS bf16 (sustained) from MEASURED_PEAKS.json'
-                    if os.path.exists(os.path.join(ROOT, 'MEASURED_PEAKS.json')) else 'peak = fallback 1.59 PFLOP/s'}
+                    'runs at 3x this rate (ceiling of frac = 1/3)'}
 
 
 def moe_roofline(net, x, peaks):
@@ -357,7 +369,7 @@ def moe_roofline(net, x, peaks):
         torch.cuda.synchronize()
     finally:
         ops.moe_assign, ops.moe_combine, ops.pack_act = o_assign, o_combine, o_pack
-    peak = peaks.get('hbm_gbs') or 6550.0
+    peak = peaks.get('hbm_gbs') or H100_HBM_GBS
     ms = sum(a.elapsed_time(b) for a, b, *_ in seq)
     by = sum(r[2] for r in seq)
     fl = sum(r[3] for r in seq)
@@ -366,6 +378,8 @@ def moe_roofline(net, x, peaks):
     out = {'bound': 'hbm', 'kernel': 'MoE dispatch+expert path (gather-pack -> grouped GEMM x2 -> combine), all MoE layers of one forward',
            'layers': len(seq), 'achieved': by / (ms * 1e-3) / 1e9 if ms else 0.0, 'peak': peak, 'unit': 'GB/s',
            'ms': ms, 'algorithmic_bytes': by, 'expert_tflops': fl / (ms * 1e-3) / 1e12 if ms else 0.0,
+           'peak_source': 'measured copy bandwidth, MEASURED_PEAKS.json' if peaks.get('hbm_gbs')
+                          else 'H100 SXM data sheet, HBM3 3.35 TB/s (not measured on this card)',
            'note': 'the expert GEMM pair is tensor-bound (16kTC^2 FLOP on 3-pass split-bf16), so the sequence cannot reach the '
                    'HBM roofline (the north-star 60 % target is NOT met on the sequence as written); dispatch_only isolates '
                    'the HBM-bound gather + scatter kernels'}
@@ -374,6 +388,27 @@ def moe_roofline(net, x, peaks):
         out['dispatch_only'] = {'achieved': dby / (dms * 1e-3) / 1e9, 'frac': dby / (dms * 1e-3) / 1e9 / peak, 'ms': dms,
                                 'algorithmic_bytes': dby}
     return out
+
+
+DUMP_SAMPLE = 1 << 21        # elements kept of a larger array (8 MB in float32): 4 feature maps + gradients < 64 MB
+
+
+def dump_sample(t):
+    """t flattened to float32; more than DUMP_SAMPLE elements are reduced to a fixed sample (seeded sorted indices that
+    depend only on the size)."""
+    t = t.detach().reshape(-1)
+    if t.numel() <= DUMP_SAMPLE:
+        return t.float()
+    g = torch.Generator(device='cpu')
+    g.manual_seed(t.numel())
+    return t[torch.randint(0, t.numel(), (DUMP_SAMPLE,), generator=g).sort().values.to(t.device)].float()
+
+
+def dump_outputs(d, arrays):
+    import numpy as np
+    os.makedirs(d, exist_ok=True)
+    for name, t in arrays.items():
+        np.save(os.path.join(d, f'{name}.npy'), t.cpu().numpy())
 
 
 def build_model(args, world, ep, ddp=True):
@@ -419,7 +454,8 @@ def run_ours(args):
     if world > 1:
         dist.init_process_group('nccl')
     lib = _lib.load()
-    assert lib.sm3_device_supported() == 1, 'bench.py needs an sm_100 (B200) device'
+    assert lib.sm3_device_supported() == 1, 'bench.py needs an sm_90 (H100) device'
+    torch.manual_seed(1234 + rank)               # noisy gating draws its noise on the device: same inputs every run
     c, B, MB, scaling, ep = resolve(args, world)
     # gradient sync: DDP's bucketed all-reduce hooks (eager launches), or ONE flat all-reduce at the end of the step, which
     # is capturable in the CUDA graph together with the whole forward+backward (sm3det_b200/graphed.py)
@@ -436,9 +472,16 @@ def run_ours(args):
     host_x = make_images(B, S, S, seed=1234 + rank).pin_memory()
     dev_x = host_x.cuda()
 
+    # --dump-outputs: references to each micro-batch's results (no extra work in the step; under CUDA-graph capture these
+    # are the graph's static outputs, which every replay rewrites)
+    last = {'outs': [], 'loss': []}
+
     def micro_step(x):
         with torch.autocast('cuda', dtype=torch.bfloat16, enabled=args.amp):
             outs, loss = model(x)
+        if args.dump_outputs:
+            last['outs'].append([o.detach() for o in outs])
+            last['loss'].append(loss.detach())
         tot = (sum(o.float().mean() for o in outs) + loss) / n_micro
         tot.backward()
         return tot.detach()
@@ -447,6 +490,7 @@ def run_ours(args):
         """one optimizer step's worth of work: fwd+bwd over the per-GPU batch, gradients accumulated over the micro-batches,
         all-reduced (DDP) once, during the last micro-batch's backward"""
         tot = None
+        last['outs'], last['loss'] = [], []
         for i in range(n_micro):
             sync_ctx = model.no_sync() if (world > 1 and not flat_sync and (i + 1 < n_micro or args.no_grad_sync)) else contextlib.nullcontext()
             with sync_ctx:
@@ -543,12 +587,23 @@ def run_ours(args):
         if i > 0:
             res_ready[cur ^ 1].synchronize()
             acc += float(host_res[cur ^ 1])
-        after_step()
+        if not (args.dump_outputs and i + 1 == args.steps):      # keep the last step's gradients for the dump
+            after_step()
     res_ready[(args.steps - 1) & 1].synchronize()
     acc += float(host_res[(args.steps - 1) & 1])
     e3.record()
     sync()
     clocks = sampler.stop() if rank == 0 else None
+    if args.dump_outputs:
+        if rank == 0:
+            arrays = {f'out{i}': dump_sample(torch.cat([m[i] for m in last['outs']])) for i in range(len(last['outs'][0]))}
+            arrays['gate_loss'] = torch.stack(last['loss']).float()
+            arrays['step_value'] = dump_sample(tot)
+            grads = [p.grad.reshape(-1) for p in net.parameters() if p.grad is not None]
+            if grads:
+                arrays['grad_sample'] = dump_sample(torch.cat(grads))
+            dump_outputs(args.dump_outputs, arrays)
+        after_step()
     if ep:
         net._ep_ctx.check()                      # expert-side capacity was never exceeded (reads a device flag; off the clock)
     ms_e2e = e2.elapsed_time(e3) / args.steps
@@ -583,18 +638,12 @@ def run_ours(args):
                 torch.cuda.synchronize()
             roof = gemm_roofline(one, peaks)
             net.zero_grad(set_to_none=True)
-            try:   # measured DRAM traffic of the tensor-core launches of one micro-batch (ncu dram__bytes_read+write, profiles/)
-                tr = json.load(open(os.path.join(ROOT, 'profiles', 'r02_gemm_traffic.json')))
-                roof['traffic'] = tr['bytes_per_launch']
-                roof['traffic_note'] = tr['note']
-            except Exception:
-                pass
             if c['family'] == 'convnext':
                 roof_moe = moe_roofline(net, xm, peaks)
         line = {'metric': METRIC, 'value': B * world / (ms * 1e-3), 'unit': 'img/s', 'n_gpus': world, 'steps': args.steps,
                 'warmup': args.warmup, 'ms_per_step': ms, 'higher_is_better': True, 'scaling': scaling, 'vs_baseline': None,
                 'dtype': ('bf16 GEMM operands (single pass), fp32 accumulate and fp32 elsewhere -- optional AMP recipe, not the headline'
-                          if args.amp else 'f32 (bf16 hi+lo split operands on tcgen05, fp32 accumulate; SIMT fp32 elsewhere)'),
+                          if args.amp else 'f32 (bf16 hi+lo split operands on wgmma, fp32 accumulate; SIMT fp32 elsewhere)'),
                 'data': 'synthetic', 'config': workload_config(args, world), 'clocks': clocks,
                 'e2e': {'value': B * world / (ms_e2e * 1e-3), 'unit': 'img/s', 'h2d_bytes_per_step': h2d,
                         'd2h_bytes_per_step': 4, 'ms_per_step': ms_e2e},
@@ -627,7 +676,7 @@ def run_ours(args):
     if world > 1:
         # Tear-down order matters when the step was graph-captured: NCCL keeps a communicator alive (and ncclCommDestroy
         # blocks) while a CUDA graph that captured collectives on it exists -- measured as a hang at exit after the JSON line
-        # on 4 GPUs (profiles/r02_multi_gpu.txt).  Destroy the graph first, then leave without tearing the group down.
+        # on 4 GPUs.  Destroy the graph first, then leave without tearing the group down.
         def stamp(msg):
             print(f'[bench rank {rank}] {msg} t={time.time() - T0:.1f}s', file=sys.stderr, flush=True)
         stamp('result printed' if rank == 0 else 'timed region done')

@@ -1,4 +1,4 @@
-/* sm3det_b200 -- C ABI of the B200 (sm_100a) kernel library behind SM3Det's ConvNeXt-MoE backbone.
+/* sm3det_b200 -- C ABI of the H100 (sm_90a) kernel library behind SM3Det's ConvNeXt-MoE backbone.
  *
  * The reference hot path is pure Python/PyTorch (mmrotate/models/backbones/convnext_moe.py); it has
  * no FFI of its own.  The closest analogue of this boundary is the `mmcv._ext` extension built at
@@ -39,8 +39,8 @@ const char* sm3_last_error(void);
 int sm3_device_supported(void);
 
 /* ---- tensor-core GEMM ------------------------------------------------------------------------
- * D[M,N] = epilogue( sum_k A(m,k) * B(n,k) ), fp32 in HBM, split-bf16 (hi+lo) operands on tcgen05,
- * fp32 accumulation in TMEM (product error ~1e-5 relative).
+ * D[M,N] = epilogue( sum_k A(m,k) * B(n,k) ), fp32 in HBM, split-bf16 (hi+lo) operands on wgmma,
+ * fp32 register accumulation (product error ~1e-5 relative).
  * Replaces: FFN.forward nn.Linear/GELU/nn.Linear (convnext_moe.py:397-405), the expert loop
  * (:244) with its gather x[_batch_index] (:265), the 2x2/s2 downsample Conv2d (:549-558), and the
  * dgrad / wgrad GEMMs autograd derives for them.
@@ -110,7 +110,7 @@ size_t sm3_gemm_workspace_bytes(const sm3_gemm_args* args);
 
 /* ---- fused dense FFN for the narrow stages (C <= 192 forward, C <= 128 backward into dv) ------------------------------
  * The [M, 4C] hidden tensor is produced and consumed on chip (GEMM1 -> +b1 -> GELU -> bf16 hi/lo split -> shared memory ->
- * GEMM2 with the accumulators in TMEM).  Replaces FFN.forward (convnext_moe.py:397-405) + layer scale / drop-path /
+ * GEMM2 with register accumulators).  Replaces FFN.forward (convnext_moe.py:397-405) + layer scale / drop-path /
  * shortcut (:367-370) of dense ConvNeXt blocks.
  *   mode 0 (forward)     out = resid + row_scale * col_scale * (gelu(A1 Wa1^T + b1) Wb^T + bias2);  aux_out = pre-scale value;
  *                        h_out (optional) = A1 Wa1^T + b1, stored once for the GEMM-based backward
@@ -134,7 +134,7 @@ typedef struct sm3_ffn_args {
 } sm3_ffn_args;
 int32_t sm3_ffn_fused_chunk(int32_t mode, int32_t C);   /* hidden chunk width for (mode, C); 0 = shape not supported */
 int sm3_ffn_fused(const sm3_ffn_args* args, void* stream);
-size_t sm3_ffn_fused_workspace_bytes(const sm3_ffn_args* args);   /* 0: accumulators live in TMEM, operands in smem */
+size_t sm3_ffn_fused_workspace_bytes(const sm3_ffn_args* args);   /* 0: accumulators live in registers, operands in smem */
 
 /* ---- LayerNorm over channels (F.layer_norm, eps inside rsqrt, biased variance) ---------------
  * Replaces LayerNorm2d.forward (convnext_moe.py:34-47) at :351 (block norm), :549-551 (downsample

@@ -164,3 +164,67 @@ def lsk_injections(cfg, gold):
     if cfg.drop_rate > 0 and gold['mode'] != 'eval':
         drops = make_drop_masks(dshapes, cfg.drop_rate)
     return noise, drops
+
+
+GOLDEN_FILE_LIMIT = 1000 * 1024     # a fixture file above this keeps its large entries in parts/
+GOLDEN_PART_LIMIT = 900 * 1024      # target size of one part
+
+
+def _nbytes(obj):
+    import io
+    b = io.BytesIO()
+    torch.save(obj, b)
+    return b.tell()
+
+
+def save_golden(gold, path):
+    """Write a fixture of tests/golden, read back by load_golden.  Above GOLDEN_FILE_LIMIT, every entry over 32 KiB moves to
+    parts/<name>.<i>.pt (dicts and lists cut into parts of at most GOLDEN_PART_LIMIT) and the file lists them under 'parts'."""
+    import glob
+    import os
+    d, name = os.path.dirname(path), os.path.basename(path)[:-3]
+    os.makedirs(d, exist_ok=True)
+    for old in glob.glob(os.path.join(d, 'parts', f'{name}.*.pt')):
+        os.remove(old)
+    if _nbytes(gold) <= GOLDEN_FILE_LIMIT:
+        torch.save(gold, path)
+        return
+    big = [k for k, v in gold.items() if _nbytes(v) > 32 * 1024]
+    base = {k: v for k, v in gold.items() if k not in big}
+    chunks = []
+    for k in big:
+        v = gold[k]
+        if isinstance(v, (dict, list)) and _nbytes(v) > GOLDEN_PART_LIMIT:
+            items = list(v.items()) if isinstance(v, dict) else list(v)
+            cur = []
+            for it in items:
+                cur.append(it)
+                if _nbytes(dict(cur) if isinstance(v, dict) else cur) > GOLDEN_PART_LIMIT:
+                    cur.pop()
+                    chunks.append({k: dict(cur) if isinstance(v, dict) else cur})
+                    cur = [it]
+            chunks.append({k: dict(cur) if isinstance(v, dict) else cur})
+        else:
+            chunks.append({k: v})
+    os.makedirs(os.path.join(d, 'parts'), exist_ok=True)
+    base['parts'] = []
+    for i, c in enumerate(chunks):
+        torch.save(c, os.path.join(d, 'parts', f'{name}.{i}.pt'))
+        base['parts'].append(f'{name}.{i}.pt')
+    torch.save(base, path)
+
+
+def load_golden(path):
+    """Load a fixture of tests/golden written by save_golden: parts are merged back (dict and list entries split over
+    several parts are joined)."""
+    import os
+    gold = torch.load(path, weights_only=False)
+    for part in gold.pop('parts', []):
+        for k, v in torch.load(os.path.join(os.path.dirname(path), 'parts', part), weights_only=False).items():
+            if isinstance(v, dict) and isinstance(gold.get(k), dict):
+                gold[k].update(v)
+            elif isinstance(v, list) and isinstance(gold.get(k), list):
+                gold[k].extend(v)
+            else:
+                gold[k] = v
+    return gold

@@ -1,6 +1,6 @@
 """Generate tests/golden/*.pt by running the UNMODIFIED reference (via oracle/ref_shim.py).
 
-Run in the build container only (needs /root/reference):  python -m oracle.gen_golden
+Needs the reference tree (SM3DET_REFERENCE_ROOT):  python -m oracle.gen_golden [case ...]   or   python -m oracle.gen_golden live
 Every case also asserts that the restated oracle reproduces the reference bit-for-bit on CPU
 (forward outputs, gate loss, routing decisions, parameter gradients) -- this is what pins the
 oracle.  Fixtures hold no weights: those are regenerated from seeds by sm3det_b200.synth.
@@ -12,7 +12,7 @@ import torch
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 from oracle import ref_shim                                   # noqa: E402
-from oracle.cases import CASES, make_noise, summarize_grad, upstream_grads   # noqa: E402
+from oracle.cases import CASES, make_noise, save_golden, summarize_grad, upstream_grads   # noqa: E402
 from oracle.convnext_moe_oracle import OracleConfig, backbone_forward, param_shapes, tie_da_weights  # noqa: E402
 from sm3det_b200.synth import make_images, make_state_dict, state_dict_checksum    # noqa: E402
 
@@ -132,8 +132,8 @@ def run_case(name, spec):
         gold['grads'] = grads
     os.makedirs(OUT, exist_ok=True)
     path = os.path.join(OUT, name + '.pt')
-    torch.save(gold, path)
-    print(f'{name}: ok, {os.path.getsize(path) / 1024:.0f} KiB, moe layers {len(record)}')
+    save_golden(gold, path)
+    print(f'{name}: ok, moe layers {len(record)}')
 
 
 def run_lsk_case(name, spec):
@@ -227,13 +227,89 @@ def run_lsk_case(name, spec):
         gold['bn'] = {k: v.clone() for k, v in bn_state.items()}
     os.makedirs(OUT, exist_ok=True)
     path = os.path.join(OUT, name + '.pt')
-    torch.save(gold, path)
-    print(f'{name}: ok, {os.path.getsize(path) / 1024:.0f} KiB, moe layers {len(record)}')
+    save_golden(gold, path)
+    print(f'{name}: ok, moe layers {len(record)}')
+
+
+# kwargs of the state_dict-layout checks in tests/test_contract.py (tiny arch: the reference cannot be built on 'meta')
+LAYOUT_CASES = {
+    'tiny_dense_multi': ('ConvNeXt_moe_MultiInput', dict(arch='tiny')),
+    'tiny_e8k2_multi': ('ConvNeXt_moe_MultiInput', dict(arch='tiny', MoE_Block_inds=[[], [], [0, 2, 4, 6, 8], [0, 2]], num_experts=8, top_k=2)),
+    'tiny_e8k3_plain': ('ConvNeXt_moe', dict(arch='tiny', MoE_Block_inds=[[], [], [0, 2, 4, 6, 8], [0, 2]], num_experts=8, top_k=3)),
+}
+LSK_S_KW = dict(MoE_Block_inds_fc1=[[], [0], [0, 2], [0]], MoE_Block_inds_fc2=[[], [0], [0, 2], [0]], num_experts=4, top_k=2,
+                embed_dims=[64, 128, 320, 512], depths=[2, 2, 4, 2], drop_rate=0.1, drop_path_rate=0.,
+                norm_cfg=dict(type='SyncBN', requires_grad=True))          # configs/SM3Det/SM3Det_lsk_s.py:13-25
+VAN_KW = dict(MoE_Block_inds_fc1=[[], [0], [0], []], MoE_Block_inds_fc2=[[], [0], [0], []], num_experts=2, top_k=1,
+              embed_dims=[32, 64, 160, 256], depths=[1, 1, 2, 1])
+FPN_KW = dict(in_channels=[96, 192, 384, 768], out_channels=256, extra_level=1, add_extra_convs='on_output', num_outs=5)
+
+
+def fpn_inputs(n=2, s=64, seed=3):
+    g = torch.Generator().manual_seed(seed)
+    return [torch.randn(n, c, s // (4 * 2 ** i), s // (4 * 2 ** i), generator=g) for i, c in enumerate(FPN_KW['in_channels'])]
+
+
+def run_live_reference():
+    """tests/golden/live/reference.pt: what the unmodified reference modules return for the small live-comparison cases
+    (forward outputs, state_dict layouts, parameter names), so the tests compare against it without the reference tree."""
+    from oracle.cases import LSK_CASES
+    from oracle.fpn_oracle import fpn_param_shapes
+    from oracle.lsk_moe_oracle import LskConfig, lsk_param_shapes
+    gold = {'convnext': {}, 'layout': {}}
+    for name in ('mini_moe_e4k2_eval', 'mini_moe_e8k3_eval'):
+        kw = dict(CASES[name]['kw'])
+        net = ref_shim.build_reference_backbone('ConvNeXt_moe_MultiInput', seed=0, **kw)
+        net.load_state_dict(make_state_dict(param_shapes(OracleConfig(**kw)), 3, True), strict=True)
+        net.eval()
+        with torch.no_grad():
+            outs, loss = net(make_images(2, 64, 64, seed=5))
+        gold['convnext'][name] = dict(outs=[o.clone() for o in outs], loss=loss.clone())
+    kw = dict(arch=dict(depths=[1, 1, 2, 1], channels=[32, 64, 96, 128]), MoE_Block_inds=[[], [], [1], []], num_experts=4, top_k=2)
+    net = ref_shim.build_reference_backbone('ConvNeXt_moe', seed=0, **kw)
+    keys = sorted(net.state_dict())
+    net.load_state_dict(make_state_dict(param_shapes(OracleConfig(multi_input=False, **kw)), 1, True), strict=True)
+    net.eval()
+    with torch.no_grad():
+        outs = net(make_images(1, 64, 64, seed=2))[0]
+    gold['convnext_plain'] = dict(keys=keys, outs=[o.clone() for o in outs])
+    spec = LSK_CASES['lsk_mini_moe_e4k2_eval']
+    mod = ref_shim.load_reference_module('lsk_moe')
+    torch.manual_seed(0)
+    net = mod.LSKNet_moe_MultiInput(norm_cfg=dict(type='SyncBN', requires_grad=True), **spec['kw'])
+    net.load_state_dict(make_state_dict(lsk_param_shapes(LskConfig(**spec['kw'])), 0, True), strict=True)
+    net.eval()
+    with torch.no_grad():
+        outs, loss = net(make_images(*spec['img'], seed=5))
+    gold['lsk'] = dict(outs=[o.clone() for o in outs], loss=loss.clone())
+    fpn = ref_shim.load_reference_module('Multitask_FPN', 'necks').MultitaskFPN(**FPN_KW)
+    sd = make_state_dict(fpn_param_shapes(FPN_KW['in_channels'], 256, 5, 1, 'on_output'), 5, True)
+    gold['fpn_keys'] = sorted(fpn.state_dict())
+    fpn.load_state_dict(sd, strict=True)
+    with torch.no_grad():
+        gold['fpn'] = {0: [o.clone() for o in fpn(fpn_inputs())],
+                       1: [o.clone() for o in fpn(fpn_inputs(), start_level=1, add_extra_convs='on_output')]}
+    for case, (cls, kw) in LAYOUT_CASES.items():
+        net = ref_shim.build_reference_backbone(cls, **kw)
+        gold['layout'][case] = dict(shapes={k: tuple(v.shape) for k, v in net.state_dict().items()},
+                                    params=sorted(n for n, _ in net.named_parameters()))
+    net = ref_shim.build_reference_backbone('ConvNeXt_DA_MultiInput', module='convnext_moe_DA', arch='tiny', drop_path_rate=0.1, datasets=None)
+    gold['layout']['da_tiny'] = dict(keys=list(net.state_dict()), params=[n for n, _ in net.named_parameters()])
+    for case, net in (('lsk_s', mod.LSKNet_moe_MultiInput(**LSK_S_KW)),
+                      ('van', ref_shim.load_reference_module('van_moe').VAN_moe_MultiInput(**VAN_KW))):
+        sd = net.state_dict()
+        gold['layout'][case] = dict(keys=sorted(sd), shapes={k: tuple(v.shape) for k, v in sd.items()})
+    path = os.path.join(OUT, 'live', 'reference.pt')
+    save_golden(gold, path)
+    print('live reference: ok')
 
 
 if __name__ == '__main__':
     from oracle.cases import LSK_CASES
     torch.set_num_threads(8)
+    if sys.argv[1:] == ['live']:
+        run_live_reference()
+        sys.exit(0)
     names = sys.argv[1:] or (list(CASES) + list(LSK_CASES))
     for nm in names:
         if nm in LSK_CASES:

@@ -1,4 +1,4 @@
-"""sm3det_b200 -- B200-native (sm_100a) implementation of SM3Det's grid-level sparse-MoE ConvNeXt backbone."""
+"""sm3det_b200 -- H100-native (sm_90a) implementation of SM3Det's grid-level sparse-MoE ConvNeXt backbone."""
 from .backbone import ConvNeXt_DA_MultiInput, ConvNeXt_moe, ConvNeXt_moe_MultiInput  # noqa: F401
 from .lsk_backbone import LSKNet_moe, LSKNet_moe_MultiInput, VAN_moe, VAN_moe_MultiInput  # noqa: F401
 from .registry import ROTATED_BACKBONES, build_backbone, register_into_mmrotate  # noqa: F401

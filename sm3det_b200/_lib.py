@@ -2,7 +2,7 @@
 
 The library is built in-tree (``make`` or ``__graft_entry__.build()``) as
 ``sm3det_b200/lib/libsm3det_b200.so``.  There is NO fallback: if the library is missing or the
-device is not sm_100, calling any op raises -- the product path never silently runs on PyTorch/CPU.
+device is not sm_90, calling any op raises -- the product path never silently runs on PyTorch/CPU.
 """
 import ctypes as C
 import os

@@ -325,7 +325,7 @@ class ConvNeXt_moe(BaseModule):
         self.num_experts = num_experts
         self.frozen_stages = frozen_stages
         self.gap_before_final_norm = gap_before_final_norm
-        self.with_cp = with_cp     # activation checkpointing is not needed at 180 GB; accepted and ignored
+        self.with_cp = with_cp     # accepted and ignored: no activation checkpointing (split large batches into passes instead)
         self.stem_patch_size = stem_patch_size
         self.norm_eps = norm_cfg.get('eps', 1e-5)
 
@@ -399,7 +399,7 @@ class ConvNeXt_moe(BaseModule):
     @staticmethod
     def _check_input(x):
         if not x.is_cuda:
-            raise RuntimeError('sm3det_b200 backbones run on CUDA (sm_100a) only; there is no CPU path')
+            raise RuntimeError('sm3det_b200 backbones run on CUDA (sm_90a) only; there is no CPU path')
         if x.dim() != 4 or x.shape[2] % 32 != 0 or x.shape[3] % 32 != 0:
             raise ValueError(f'expected [N,3,H,W] with H, W multiples of 32 (Pad size_divisor=32), got {tuple(x.shape)}')
 

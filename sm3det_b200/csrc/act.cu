@@ -1,7 +1,7 @@
 // Fused activation + operand pre-split ("act_pack").
 //
 // The FFN hidden tensor h = W1 v + b1 is the largest activation of a block ([rows, 4C]).  Evaluating GELU / GELU'
-// in the GEMM epilogue (128 or 256 threads per SM) is instruction-issue bound (profiles/r01_gemm_allpacked_ffn1_stage0.txt),
+// in the GEMM epilogue (256 threads per SM) is instruction-issue bound,
 // so the GEMM only stores h and this HBM-bound elementwise kernel -- full occupancy, 8 elements per thread -- applies
 // the activation AND writes the result directly as the pre-split bf16 hi/lo tile images the next GEMMs bulk-copy:
 //   mode 0  y = gelu(h)            forward:  A operand of GEMM2 (K-major image);  backward: B operand of wgrad2 (MN image)

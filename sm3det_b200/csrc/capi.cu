@@ -15,10 +15,11 @@ int sm3_abi_version(void) { return SM3_ABI_VERSION; }
 const char* sm3_last_error(void) { return sm3::last_error(); }
 
 int sm3_device_supported(void) {
-  int dev = 0, major = 0;
+  int dev = 0, major = 0, minor = 0;
   if (cudaGetDevice(&dev) != cudaSuccess) return 0;
   if (cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, dev) != cudaSuccess) return 0;
-  return major == 10 ? 1 : 0;
+  if (cudaDeviceGetAttribute(&minor, cudaDevAttrComputeCapabilityMinor, dev) != cudaSuccess) return 0;
+  return (major == 9 && minor == 0) ? 1 : 0;
 }
 
 int sm3_gemm(const sm3_gemm_args* a, void* stream) {

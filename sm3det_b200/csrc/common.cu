@@ -35,12 +35,12 @@ int num_sms() {
   std::call_once(once[dev], [dev]() {
     int n = 0;
     cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
-    cached[dev] = n > 0 ? n : 148;
+    cached[dev] = n > 0 ? n : 132;
   });
   return cached[dev];
 }
 
-// Persistent tcgen05 kernels occupy a whole SM each (all of its registers / shared memory), so a collective launched on
+// Persistent GEMM kernels occupy a whole SM each (all of its registers / shared memory), so a collective launched on
 // another stream (NCCL's gradient all-reduce under DDP) cannot co-reside and is serialised behind them.  SM3_RESERVE_SMS=n
 // keeps n SMs out of the persistent grids so that NCCL's CTAs run concurrently with the backward GEMMs.
 int persistent_grid_sms() {

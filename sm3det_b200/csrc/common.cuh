@@ -1,12 +1,12 @@
-// Common helpers for the sm3det_b200 CUDA library (sm_100a only).
+// Common helpers for the sm3det_b200 CUDA library (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include <cstdio>
 #include "../../include/sm3det_b200.h"
 
-#if defined(__CUDA_ARCH__) && (__CUDA_ARCH__ < 1000)
-#error "sm3det_b200 kernels are written for sm_100a only"
+#if defined(__CUDA_ARCH__) && (__CUDA_ARCH__ != 900 || !defined(__CUDA_ARCH_FEAT_SM90_ALL))
+#error "sm3det_b200 kernels are written for sm_90a only (wgmma, setmaxnreg)"
 #endif
 
 namespace sm3 {
@@ -76,6 +76,15 @@ __device__ __forceinline__ float gelu_grad_fast(float x) {
   float Phi, e;
   phi_parts(x, Phi, e);
   return fmaf(x * 0.39894228040143267794f, e, Phi);
+}
+
+// Packed-FP32 pair: two adjacent fp32 values in one 64-bit register (low word first).  The kernels keep their
+// operands as pairs (one LDS.64 feeds two FMAs); sm_90 has no packed-fp32 FMA, so ffma2 is two IEEE fmaf.
+typedef unsigned long long f32x2_t;
+__device__ __forceinline__ f32x2_t ffma2(f32x2_t a, f32x2_t b, f32x2_t c) {
+  const float d0 = fmaf(__uint_as_float((uint32_t)a), __uint_as_float((uint32_t)b), __uint_as_float((uint32_t)c));
+  const float d1 = fmaf(__uint_as_float((uint32_t)(a >> 32)), __uint_as_float((uint32_t)(b >> 32)), __uint_as_float((uint32_t)(c >> 32)));
+  return (f32x2_t)__float_as_uint(d0) | ((f32x2_t)__float_as_uint(d1) << 32);
 }
 
 __device__ __forceinline__ float4 ldg_f4(const float* p) {

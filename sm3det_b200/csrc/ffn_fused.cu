@@ -1,5 +1,5 @@
-// Fused dense-FFN kernels (see ffn_fused.cuh for the what and why).  sm_100a only: tcgen05.mma with TMEM accumulators,
-// cp.async.bulk (TMA bulk copies) completing on mbarriers, one persistent CTA per SM.
+// Fused dense-FFN kernels (see ffn_fused.cuh for the what and why).  sm_90a only: wgmma.mma_async with register
+// accumulators, cp.async.bulk (TMA bulk copies) completing on mbarriers, one persistent CTA per SM.
 #define SM3_GEMM_KERNEL_IMPL
 #include "gemm_tc.cuh"
 #include "ffn_fused.cuh"
@@ -9,8 +9,11 @@ namespace sm3 {
 namespace ffn {
 using namespace gemm;
 
-constexpr int THREADS = 384;                 // 12 warps: 0 A/Wa producer, 1 Wb producer, 2 MMA issuer, 3 idle, 4-11 middle/epilogue
-constexpr int W_PROD_A = 0, W_PROD_B = 1, W_MMA = 2, EPI0 = 4, NE = 8;
+// 12 warps: 0 A/Wa producer, 1 Wb producer, 2-3 idle; 4-7 and 8-11 are the two consumer warpgroups, each owning 64 of
+// the tile's 128 token rows through GEMM-a, the middle stage, GEMM-b and the final epilogue.
+constexpr int THREADS = 384;
+constexpr int W_PROD_A = 0, W_PROD_B = 1, EPI0 = 4, NE = 8;
+constexpr int CONS_REGS = 232, PROD_REGS = 40;         // setmaxnreg: acc_o alone is up to 128 registers (C = 256)
 constexpr uint32_t SMEM_LIMIT = 232448u - 1024u;      // 227 KB opt-in maximum minus the 1 KB alignment slack
 constexpr uint32_t STAGING = NE * EPI_STAGE_BYTES;    // per-warp transpose staging of the final epilogue
 constexpr uint32_t BARS = 256;
@@ -35,35 +38,30 @@ __device__ __forceinline__ void sts128(uint32_t addr, uint32_t a, uint32_t b, ui
   asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(addr), "r"(a), "r"(b), "r"(c), "r"(d) : "memory");
 }
 
-// split 8 fp32 (one 16-byte operand chunk) into the hi / lo bf16 planes
-__device__ __forceinline__ void split8(const float* v, uint4& hi, uint4& lo) {
-  uint32_t h[4], l[4];
-#pragma unroll
-  for (int e = 0; e < 8; e += 2) {
-    const uint32_t u0 = __float_as_uint(v[e]), u1 = __float_as_uint(v[e + 1]);
-    h[e / 2] = __byte_perm(u0, u1, 0x7632);
-    const uint32_t r0 = __float_as_uint(v[e] - __uint_as_float(u0 & 0xFFFF0000u)) + 0x8000u;
-    const uint32_t r1 = __float_as_uint(v[e + 1] - __uint_as_float(u1 & 0xFFFF0000u)) + 0x8000u;
-    l[e / 2] = __byte_perm(r0, r1, 0x7632);
-  }
-  hi = make_uint4(h[0], h[1], h[2], h[3]);
-  lo = make_uint4(l[0], l[1], l[2], l[3]);
+// split 2 fp32 into one bf16x2 of the hi plane and one of the lo plane
+__device__ __forceinline__ void split2(float v0, float v1, uint32_t& hi, uint32_t& lo) {
+  const uint32_t u0 = __float_as_uint(v0), u1 = __float_as_uint(v1);
+  hi = __byte_perm(u0, u1, 0x7632);
+  const uint32_t r0 = __float_as_uint(v0 - __uint_as_float(u0 & 0xFFFF0000u)) + 0x8000u;
+  const uint32_t r1 = __float_as_uint(v1 - __uint_as_float(u1 & 0xFFFF0000u)) + 0x8000u;
+  lo = __byte_perm(r0, r1, 0x7632);
 }
 
 // 3-pass (or 1-pass) split-bf16 product of one 16-k step:  D (+)= (Ahi + Alo)(Bhi + Blo) minus the lo*lo term
-__device__ __forceinline__ void mma3(uint32_t d, uint64_t ahi, uint64_t alo, uint64_t bhi, uint64_t blo, uint32_t idesc,
-                                     uint32_t accum, int passes) {
+template <int N, int NA>
+__device__ __forceinline__ void mma3(float (&d)[NA], uint64_t ahi, uint64_t alo, uint64_t bhi, uint64_t blo, uint32_t accum,
+                                     int passes) {
   if (passes == 1) {
-    tc_mma(d, ahi, bhi, idesc, accum);
+    wg::mma<N, 0, 0>(d, ahi, bhi, accum);
   } else {
-    tc_mma(d, alo, bhi, idesc, accum);
-    tc_mma(d, ahi, blo, idesc, 1u);
-    tc_mma(d, ahi, bhi, idesc, 1u);
+    wg::mma<N, 0, 0>(d, alo, bhi, accum);
+    wg::mma<N, 0, 0>(d, ahi, blo, 1u);
+    wg::mma<N, 0, 0>(d, ahi, bhi, 1u);
   }
 }
 
 // ================================================================================================================
-template <int MODE, int HC>
+template <int MODE, int HC, int C>
 __global__ void __launch_bounds__(THREADS, 1) ffn_chain_kernel(const __grid_constant__ ChainK k) {
   const ChainParams& p = k.p;
   const Layout& L = k.L;
@@ -75,35 +73,21 @@ __global__ void __launch_bounds__(THREADS, 1) ffn_chain_kernel(const __grid_cons
   auto wa_empty = [&](int s) { return bar + 32u + 8u * s; };
   auto wb_full = [&](int s) { return bar + 48u + 8u * s; };
   auto wb_empty = [&](int s) { return bar + 64u + 8u * s; };
-  auto h_full = [&](int b) { return bar + 80u + 8u * b; };
-  auto h_empty = [&](int b) { return bar + 96u + 8u * b; };
-  const uint32_t act_full = bar + 112, act_empty = bar + 120, o_full = bar + 128, o_empty = bar + 136, tmem_slot = bar + 144;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   constexpr int NA = (MODE == 1) ? 2 : 1;
 
   if (threadIdx.x == 0) {
-    mbar_init(a_full, 1); mbar_init(a_empty, 1);
-    for (int s = 0; s < 2; ++s) { mbar_init(wa_full(s), 1); mbar_init(wa_empty(s), 1); mbar_init(wb_full(s), 1); mbar_init(wb_empty(s), 1); }
-    for (int b = 0; b < 2; ++b) { mbar_init(h_full(b), 1); mbar_init(h_empty(b), NE); }
-    mbar_init(act_full, NE); mbar_init(act_empty, 1); mbar_init(o_full, 1); mbar_init(o_empty, NE);
+    mbar_init(a_full, 1); mbar_init(a_empty, NE);
+    for (int s = 0; s < 2; ++s) { mbar_init(wa_full(s), 1); mbar_init(wa_empty(s), NE); mbar_init(wb_full(s), 1); mbar_init(wb_empty(s), NE); }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  if (warp == W_MMA) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(tmem_slot), "r"(512) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  uint32_t tmem_base;
-  asm volatile("ld.shared.u32 %0, [%1];" : "=r"(tmem_base) : "r"(tmem_slot) : "memory");
-  // TMEM columns: [b * NA * HC, ...) = acc_h[b] (, acc_d[b]);  acc_o behind them
-  const uint32_t col_o = 2u * NA * HC;
-  const int nch = k.nch, C = p.C;
-  const int kbc = C / 32;
+  const int nch = k.nch;
+  constexpr int kbc = C / 32;
 
-  if (warp == W_PROD_A) {
-    if (lane == 0) {
+  if (warp < EPI0) {
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(PROD_REGS));
+    if (warp == W_PROD_A && lane == 0) {
       uint32_t n_t = 0, n_w = 0;
       for (int t = blockIdx.x; t < k.m_tiles; t += gridDim.x, ++n_t) {
         mbar_wait(a_empty, (n_t & 1u) ^ 1u);
@@ -122,9 +106,7 @@ __global__ void __launch_bounds__(THREADS, 1) ffn_chain_kernel(const __grid_cons
           if (MODE == 1) bulk_g2s(dst + L.wa_chunk, reinterpret_cast<const uint8_t*>(p.wa2) + (long long)j * L.wa_chunk, L.wa_chunk, wa_full(s));
         }
       }
-    }
-  } else if (warp == W_PROD_B) {
-    if (lane == 0) {
+    } else if (warp == W_PROD_B && lane == 0) {
       uint32_t n = 0;
       for (int t = blockIdx.x; t < k.m_tiles; t += gridDim.x) {
         for (int j = 0; j < nch; ++j, ++n) {
@@ -136,157 +118,129 @@ __global__ void __launch_bounds__(THREADS, 1) ffn_chain_kernel(const __grid_cons
         }
       }
     }
-  } else if (warp == W_MMA) {
-    if (lane == 0) {
-      const uint32_t idesc_a = make_instr_desc(HC, false, false), idesc_b = make_instr_desc(C, false, false);
-      uint32_t n_t = 0, n_c = 0, n_b = 0;
-      for (int t = blockIdx.x; t < k.m_tiles; t += gridDim.x, ++n_t) {
-        mbar_wait(a_full, n_t & 1u);
-        tc_fence_after();
-        for (int step = 0; step <= nch; ++step) {
-          if (step < nch) {
-            const int b = n_c & 1, s = n_c % L.sa;
-            mbar_wait(h_empty(b), ((n_c >> 1) & 1u) ^ 1u);
-            mbar_wait(wa_full(s), (n_c / L.sa) & 1u);
-            tc_fence_after();
-            const uint32_t wst = sb0 + L.wa + s * L.wa_stage;
-            // the single issuing thread is the bottleneck of these narrow MMAs (N = 32..96 is 16..48 tensor cycles each):
-            // descriptors are built once per operand block and only ADVANCED inside the loops (address field, 16-byte units)
-#pragma unroll
-            for (int g = 0; g < NA; ++g) {
-              const uint32_t acc = tmem_base + (uint32_t)((b * NA + g) * HC);
-              uint64_t da = make_smem_desc(sb0 + L.a + g * L.a_tile, false), db = make_smem_desc(wst + g * L.wa_chunk, false);
-              for (int kb = 0; kb < kbc; ++kb) {
-                mma3(acc, da, da + 512u, db, db + HC * 4u, idesc_a, kb > 0 ? 1u : 0u, p.passes);
-                mma3(acc, da + 2u, da + 514u, db + 2u, db + HC * 4u + 2u, idesc_a, 1u, p.passes);
-                da += 1024u; db += HC * 8u;
-              }
-            }
-            tc_commit(wa_empty(s));
-            tc_commit(h_full(b));
-            if (step == nch - 1) tc_commit(a_empty);
-            ++n_c;
-          }
-          if (step >= 1) {
-            const int jb = step - 1, s = n_b % L.sb;
-            if (jb == 0) mbar_wait(o_empty, (n_t & 1u) ^ 1u);
-            mbar_wait(act_full, n_b & 1u);
-            mbar_wait(wb_full(s), (n_b / L.sb) & 1u);
-            tc_fence_after();
-            const uint32_t acc = tmem_base + col_o;
-            uint64_t da = make_smem_desc(sb0 + L.act, false), db = make_smem_desc(sb0 + L.wb + s * L.wb_stage, false);
-            const uint64_t blo = (uint64_t)(C * 4);              // lo plane of a Wb k-block: C * 64 bytes behind the hi plane
-#pragma unroll
-            for (int kb = 0; kb < HC / 32; ++kb) {
-              mma3(acc, da, da + 512u, db, db + blo, idesc_b, (jb > 0 || kb > 0) ? 1u : 0u, p.passes);
-              mma3(acc, da + 2u, da + 514u, db + 2u, db + blo + 2u, idesc_b, 1u, p.passes);
-              da += 1024u; db += 2u * blo;
-            }
-            tc_commit(wb_empty(s));
-            tc_commit(act_empty);
-            if (jb == nch - 1) tc_commit(o_full);
-            ++n_b;
-          }
-        }
-      }
-    }
-  } else if (warp >= EPI0) {
-    // ------------------------------ middle stage + final epilogue -------------------------------------------
-    const int e = warp - EPI0, q = warp & 3, half = e >> 2;
-    constexpr int HCW = HC / 2;                         // hidden columns of a chunk handled by this warp
-    const int c0 = half * HCW;
-    const uint32_t lane_t = (uint32_t)(q * 32) << 16;
-    const uint32_t r = (uint32_t)(q * 32 + lane);       // token row inside the tile = TMEM lane
+  } else {
+    asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(CONS_REGS));
+    // ------------------------------ consumers: GEMM-a, middle stage, GEMM-b, final epilogue -----------------------
+    const int e = warp - EPI0, g = e >> 2, wq = warp & 3;
+    const uint32_t slab = (uint32_t)g * WG_A_BYTES;              // this warpgroup's 64 rows inside a 128-row operand plane
     const uint32_t stage_base = sb0 + L.stage + (uint32_t)e * EPI_STAGE_BYTES;
     const int rl = lane >> 2, c4 = (lane & 3) * 4;
-    const int nchunks = C / 16;
-    uint32_t n_c = 0, n_t = 0;
+    const int r_lo = g * 64 + wq * 16 + rl;                      // tile rows of this thread's fragment: r_lo, r_lo + 8
+    auto wg_bar = [&]() { asm volatile("bar.sync %0, 128;" ::"r"(1 + g) : "memory"); };
+    float acc_h[HC / 2], acc_d[HC / 2], acc_o[C / 2];
+    uint32_t n_c = 0, n_b = 0, n_t = 0;
+    auto gemm_a = [&](uint32_t nc) {                              // acc_h (, acc_d) = A1 (, A2) . Wa_j^T over K = C
+      const int s = nc % L.sa;
+      mbar_wait(wa_full(s), (nc / L.sa) & 1u);
+      const uint32_t wst = sb0 + L.wa + s * L.wa_stage;
+#pragma unroll
+      for (int q = 0; q < NA; ++q) {
+        uint64_t da = make_smem_desc(sb0 + L.a + q * L.a_tile + slab, false), db = make_smem_desc(wst + q * L.wa_chunk, false);
+        for (int kb = 0; kb < kbc; ++kb) {
+          if (q == 0) {
+            mma3<HC>(acc_h, da, da + 512u, db, db + HC * 4u, kb > 0 ? 1u : 0u, p.passes);
+            mma3<HC>(acc_h, da + 2u, da + 514u, db + 2u, db + HC * 4u + 2u, 1u, p.passes);
+          } else {
+            mma3<HC>(acc_d, da, da + 512u, db, db + HC * 4u, kb > 0 ? 1u : 0u, p.passes);
+            mma3<HC>(acc_d, da + 2u, da + 514u, db + 2u, db + HC * 4u + 2u, 1u, p.passes);
+          }
+          da += 1024u; db += HC * 8u;
+        }
+      }
+    };
     for (int t = blockIdx.x; t < k.m_tiles; t += gridDim.x, ++n_t) {
+      mbar_wait(a_full, n_t & 1u);
+      wg::fence();
+      gemm_a(n_c);
+      wg::commit();
       for (int j = 0; j < nch; ++j, ++n_c) {
-        const int b = n_c & 1;
-        mbar_wait(h_full(b), (n_c >> 1) & 1u);
-        tc_fence_after();
-        uint32_t rh[HCW], rd[HCW];
-        const uint32_t th = tmem_base + lane_t + (uint32_t)((b * NA) * HC + c0);
-#pragma unroll
-        for (int g = 0; g < HCW / 16; ++g) {
-          tc_ld16_issue(th + g * 16, *reinterpret_cast<uint32_t(*)[16]>(&rh[g * 16]));
-          if constexpr (MODE == 1) tc_ld16_issue(th + HC + g * 16, *reinterpret_cast<uint32_t(*)[16]>(&rd[g * 16]));
-        }
-        tc_wait_ld();
-        tc_fence_before();
+        // GEMM-a(j) and GEMM-b(j-1) are complete: hand their operand stages back
+        wg::wait<0>();
+        wg::fence_operand(acc_h);
+        if constexpr (MODE == 1) wg::fence_operand(acc_d);
         __syncwarp();
-        if (lane == 0) mbar_arrive(h_empty(b));
-        float y[HCW];
-        const float* b1 = p.bias1 + (long long)j * HC + c0;
-        // training forward: the pre-activation h = A1 Wa1^T + b1 is stored once (fp32, row-major) for the GEMM-based
-        // backward; each lane owns one token row and writes HCW * 4 contiguous bytes of it (whole 128-byte lines)
-        float* hrow = nullptr;
-        if (MODE == 0 && p.h_out) {
-          const long long row = (long long)t * 128 + r;
-          if (row < p.M) hrow = p.h_out + row * p.H4 + (long long)j * HC + c0;
+        if (lane == 0) {
+          mbar_arrive(wa_empty(n_c % L.sa));
+          if (j > 0) mbar_arrive(wb_empty((n_b - 1) % L.sb));
+          if (j == nch - 1) mbar_arrive(a_empty);
         }
+        // middle: y = gelu(h) or dz-side * gelu'(h), split hi/lo into the K-major SWIZZLE_64B image of GEMM-b's A operand
+        const float* b1 = p.bias1 + (long long)j * HC;
 #pragma unroll
-        for (int i = 0; i < HCW; i += 4) {
-          const float4 bv = ldg_f4(b1 + i);
-          const float bb[4] = {bv.x, bv.y, bv.z, bv.w};
-          if (MODE == 0 && hrow)
-            *reinterpret_cast<float4*>(hrow + i) = make_float4(__uint_as_float(rh[i]) + bb[0], __uint_as_float(rh[i + 1]) + bb[1],
-                                                               __uint_as_float(rh[i + 2]) + bb[2], __uint_as_float(rh[i + 3]) + bb[3]);
+        for (int q = 0; q < HC / 8; ++q) {
+          const int kk = 8 * q + 2 * (lane & 3);
+          const float2 bv = __ldg(reinterpret_cast<const float2*>(b1 + kk));
 #pragma unroll
-          for (int u = 0; u < 4; ++u) {
-            const float x = __uint_as_float(rh[i + u]) + bb[u];
-            if (p.debug & 1) y[i + u] = x;
-            else if constexpr (MODE == 0) y[i + u] = gelu_fast(x);
-            else y[i + u] = __uint_as_float(rd[i + u]) * gelu_grad_fast(x);
+          for (int h = 0; h < 2; ++h) {
+            const int r = r_lo + 8 * h;
+            const float x0 = acc_h[4 * q + 2 * h] + bv.x, x1 = acc_h[4 * q + 2 * h + 1] + bv.y;
+            // training forward: the pre-activation h = A1 Wa1^T + b1 is stored once (fp32, row-major) for the GEMM-based backward
+            if (MODE == 0 && p.h_out) {
+              const long long row = (long long)t * 128 + r;
+              if (row < p.M) *reinterpret_cast<float2*>(p.h_out + row * p.H4 + (long long)j * HC + kk) = make_float2(x0, x1);
+            }
+            float y0, y1;
+            if (p.debug & 1) { y0 = x0; y1 = x1; }
+            else if constexpr (MODE == 0) { y0 = gelu_fast(x0); y1 = gelu_fast(x1); }
+            else { y0 = acc_d[4 * q + 2 * h] * gelu_grad_fast(x0); y1 = acc_d[4 * q + 2 * h + 1] * gelu_grad_fast(x1); }
+            if (p.debug & 2) continue;
+            uint32_t hi, lo;
+            split2(y0, y1, hi, lo);
+            const uint32_t o = sb0 + L.act + (uint32_t)(kk >> 5) * 16384u + kmajor_sw64_offset((uint32_t)r, (uint32_t)((kk & 31) >> 3)) +
+                               (uint32_t)(kk & 7) * 2u;
+            asm volatile("st.shared.b32 [%0], %1;" ::"r"(o), "r"(hi) : "memory");
+            asm volatile("st.shared.b32 [%0], %1;" ::"r"(o + 8192u), "r"(lo) : "memory");
           }
         }
-        mbar_wait(act_empty, (n_c & 1u) ^ 1u);          // GEMM-b of the previous chunk has finished reading the block
-#pragma unroll
-        for (int i = 0; i < HCW; i += 8) {
-          if (p.debug & 2) break;
-          uint4 hi, lo;
-          split8(&y[i], hi, lo);
-          const int kk = c0 + i;
-          const uint32_t o = sb0 + L.act + (uint32_t)(kk >> 5) * 16384u + kmajor_sw64_offset(r, (uint32_t)((kk & 31) >> 3));
-          sts128(o, hi.x, hi.y, hi.z, hi.w);
-          sts128(o + 8192u, lo.x, lo.y, lo.z, lo.w);
-        }
         fence_proxy_async_smem();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(act_full);
-      }
-      // ---- final epilogue of the tile: TMEM -> registers -> per-warp smem transpose -> coalesced 64-byte row segments
-      mbar_wait(o_full, n_t & 1u);
-      tc_fence_after();
-      const long long row0 = (long long)t * 128 + q * 32;
-      const uint32_t to = tmem_base + lane_t + col_o;
-      for (int c = half; c < nchunks; c += 2) {
-        uint32_t vr[16];
-        tc_ld16_issue(to + (uint32_t)(c * 16), vr);
-        const int n = c * 16 + c4;
-        float4 rr[4];
+        wg_bar();                                                 // the warpgroup's 64 activation rows are complete
+        // GEMM-b(j): acc_o += y . Wb_j^T over K = HC; GEMM-a(j+1) is issued behind it into the freed acc_h
+        const int s = n_b % L.sb;
+        mbar_wait(wb_full(s), (n_b / L.sb) & 1u);
+        wg::fence();
+        {
+          uint64_t da = make_smem_desc(sb0 + L.act + slab, false), db = make_smem_desc(sb0 + L.wb + s * L.wb_stage, false);
+          const uint64_t blo = (uint64_t)(C * 4);              // lo plane of a Wb k-block: C * 64 bytes behind the hi plane
 #pragma unroll
-        for (int it = 0; it < 4; ++it) {
+          for (int kb = 0; kb < HC / 32; ++kb) {
+            mma3<C>(acc_o, da, da + 512u, db, db + blo, (j > 0 || kb > 0) ? 1u : 0u, p.passes);
+            mma3<C>(acc_o, da + 2u, da + 514u, db + 2u, db + blo + 2u, 1u, p.passes);
+            da += 1024u; db += 2u * blo;
+          }
+        }
+        ++n_b;
+        if (j + 1 < nch) gemm_a(n_c + 1);
+        wg::commit();
+      }
+      wg::wait<0>();
+      wg::fence_operand(acc_o);
+      __syncwarp();
+      if (lane == 0) mbar_arrive(wb_empty((n_b - 1) % L.sb));
+      // ---- final epilogue of the tile: registers -> per-warp smem transpose -> coalesced 64-byte row segments
+      const long long row0 = (long long)t * 128 + g * 64 + wq * 16;
+#pragma unroll
+      for (int c = 0; c < C / 16; ++c) {
+        const int n = c * 16 + c4;
+        float4 rr[2];
+#pragma unroll
+        for (int it = 0; it < 2; ++it) {
           const long long row = row0 + it * 8 + rl;
           rr[it] = (p.resid && row < p.M) ? ldg_f4(p.resid + row * C + n) : make_float4(0.f, 0.f, 0.f, 0.f);
         }
-        tc_wait_ld();
-        if (c + 2 >= nchunks) {                          // this warp's last read of acc_o
-          tc_fence_before();
-          __syncwarp();
-          if (lane == 0) mbar_arrive(o_empty);
-        }
         __syncwarp();                                    // the previous chunk's reads of the staging rows are done
 #pragma unroll
-        for (int jj = 0; jj < 4; ++jj)
-          sts128(stage_base + (uint32_t)(lane * EPI_STAGE_ROW_FLOATS + 4 * jj) * 4u, vr[4 * jj], vr[4 * jj + 1], vr[4 * jj + 2], vr[4 * jj + 3]);
+        for (int qq = 0; qq < 2; ++qq)
+#pragma unroll
+          for (int h = 0; h < 2; ++h)
+            asm volatile("st.shared.v2.f32 [%0], {%1, %2};"
+                         ::"r"(stage_base + (uint32_t)((rl + 8 * h) * EPI_STAGE_ROW_FLOATS + 8 * qq + 2 * (lane & 3)) * 4u),
+                           "f"(acc_o[8 * c + 4 * qq + 2 * h]), "f"(acc_o[8 * c + 4 * qq + 2 * h + 1]) : "memory");
         __syncwarp();
         float4 bv = make_float4(0.f, 0.f, 0.f, 0.f), sv = make_float4(1.f, 1.f, 1.f, 1.f);
         if (p.bias2) bv = ldg_f4(p.bias2 + n);
         if (p.col_scale) sv = ldg_f4(p.col_scale + n);
 #pragma unroll
-        for (int it = 0; it < 4; ++it) {
+        for (int it = 0; it < 2; ++it) {
           const int rr_ = it * 8 + rl;
           const long long row = row0 + rr_;
           if (row >= p.M) continue;
@@ -302,13 +256,6 @@ __global__ void __launch_bounds__(THREADS, 1) ffn_chain_kernel(const __grid_cons
         }
       }
     }
-  }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == W_MMA) {
-    tc_fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(512) : "memory");
   }
 }
 
@@ -360,7 +307,6 @@ int chain(const ChainParams& p, cudaStream_t stream) {
   SM3_REQUIRE(p.HC == 32 || p.HC == 64, SM3_ERR_INVALID_ARG, "ffn chain: chunk must be 32 or 64 (sm3_ffn_fused_chunk), got %d", p.HC);
   SM3_REQUIRE(pick_chain(p.mode, p.C, p.HC, HC, k.L), SM3_ERR_UNSUPPORTED_SHAPE, "ffn chain: C=%d with chunk %d does not fit shared memory (mode %d)", p.C, p.HC, p.mode);
   SM3_REQUIRE(p.H4 % HC == 0 && p.C % 16 == 0, SM3_ERR_UNSUPPORTED_SHAPE, "ffn chain: H4=%d not a multiple of the chunk %d", p.H4, HC);
-  SM3_REQUIRE(2 * (p.mode == 1 ? 2 : 1) * HC + p.C <= 512, SM3_ERR_UNSUPPORTED_SHAPE, "ffn chain: TMEM budget");
   SM3_REQUIRE(aligned16(p.a1) && aligned16(p.wa1) && aligned16(p.wb) && aligned16(p.out) && aligned16(p.bias1) &&
               (!p.a2 || aligned16(p.a2)) && (!p.wa2 || aligned16(p.wa2)) && (!p.resid || aligned16(p.resid)) &&
               (!p.aux_out || aligned16(p.aux_out)) && (!p.bias2 || aligned16(p.bias2)) && (!p.col_scale || aligned16(p.col_scale)),
@@ -370,13 +316,22 @@ int chain(const ChainParams& p, cudaStream_t stream) {
   k.nch = p.H4 / HC;
   int grid = persistent_grid_sms();
   if (grid > k.m_tiles) grid = k.m_tiles;
-#define SM3_CHAIN_LAUNCH(MODE_, HC_)                                                                                        \
+#define SM3_CHAIN_LAUNCH(MODE_, HC_, C_)                                                                                    \
   do {                                                                                                                      \
-    cudaFuncSetAttribute(ffn_chain_kernel<MODE_, HC_>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)k.L.total);        \
-    ffn_chain_kernel<MODE_, HC_><<<grid, THREADS, k.L.total, stream>>>(k);                                                  \
+    cudaFuncSetAttribute(ffn_chain_kernel<MODE_, HC_, C_>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)k.L.total);    \
+    ffn_chain_kernel<MODE_, HC_, C_><<<grid, THREADS, k.L.total, stream>>>(k);                                              \
   } while (0)
-  if (p.mode == 0) { if (HC == 64) SM3_CHAIN_LAUNCH(0, 64); else SM3_CHAIN_LAUNCH(0, 32); }
-  else { if (HC == 64) SM3_CHAIN_LAUNCH(1, 64); else SM3_CHAIN_LAUNCH(1, 32); }
+  // the accumulator widths (HC for GEMM-a, C for GEMM-b) are wgmma shapes, i.e. template arguments
+#define SM3_CHAIN_C(MODE_, HC_)                                                                                             \
+  switch (p.C) {                                                                                                            \
+    case 32: SM3_CHAIN_LAUNCH(MODE_, HC_, 32); break;   case 64: SM3_CHAIN_LAUNCH(MODE_, HC_, 64); break;                   \
+    case 96: SM3_CHAIN_LAUNCH(MODE_, HC_, 96); break;   case 128: SM3_CHAIN_LAUNCH(MODE_, HC_, 128); break;                 \
+    case 160: SM3_CHAIN_LAUNCH(MODE_, HC_, 160); break; case 192: SM3_CHAIN_LAUNCH(MODE_, HC_, 192); break;                 \
+    case 224: SM3_CHAIN_LAUNCH(MODE_, HC_, 224); break; default: SM3_CHAIN_LAUNCH(MODE_, HC_, 256); break;                  \
+  }
+  if (p.mode == 0) { if (HC == 64) { SM3_CHAIN_C(0, 64) } else { SM3_CHAIN_C(0, 32) } }
+  else { if (HC == 64) { SM3_CHAIN_C(1, 64) } else { SM3_CHAIN_C(1, 32) } }
+#undef SM3_CHAIN_C
 #undef SM3_CHAIN_LAUNCH
   return check_launch("ffn_chain_kernel");
 }

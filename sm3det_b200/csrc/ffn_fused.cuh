@@ -7,7 +7,7 @@
 // those GEMMs are HBM streams (K or N <= 192), not tensor-bound.  Here one persistent CTA per SM walks 128-token tiles:
 //
 //   ffn_chain_kernel<MODE, HC>      per tile, per hidden chunk j of HC columns:
-//        GEMM-a   acc_h[128 x HC]  = A1 . Wa1_j^T                      (tcgen05, 3-pass split-bf16, accumulator in TMEM)
+//        GEMM-a   acc_h[128 x HC]  = A1 . Wa1_j^T                      (wgmma, 3-pass split-bf16, register accumulator)
 //        (MODE 1) acc_d[128 x HC]  = A2 . Wa2_j^T
 //        middle   MODE 0: y = gelu(acc_h + b1_j)         MODE 1: y = acc_d * gelu'(acc_h + b1_j)
 //                 -> split hi/lo -> shared memory, directly in the K-major SWIZZLE_64B operand layout
@@ -17,10 +17,7 @@
 //      RECOMPUTED, A2 = dz, Wa1 = W1, Wa2 = (gamma W2)^T, Wb = W1^T) -- the tensor pipe has >2x slack on these shapes,
 //      HBM does not, so nothing hidden-sized is saved by the forward at all.
 //
-// Not fused (measured, profiles/r02_mma_microbench.txt + r02_ffn_fused_timing.txt): the weight gradients.  A kernel that
-// recomputed h / dh per hidden slice and accumulated dW1, dW2, db1 in TMEM was written and measured at 1.9 ms per stage-0
-// block (vs ~0.4 ms for the two split-K GEMMs it would replace): with M = 128, K = 16 every tcgen05.mma costs >= 64-88 cycles
-// for its 4 KB A-operand fetch regardless of N, so N = 32..96 MMAs run the tensor pipe at 18-55 %.  It was removed.
+// Not fused: the weight gradients (split-K GEMMs).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>

@@ -1,4 +1,4 @@
-// Host launcher for the split-bf16 tcgen05 GEMM (see gemm_tc.cuh).
+// Host launcher for the split-bf16 wgmma GEMM (see gemm_tc.cuh).
 #define SM3_GEMM_KERNEL_IMPL
 #include "gemm_tc.cuh"
 #include <mutex>
@@ -8,7 +8,7 @@ const char* last_error();
 namespace gemm {
 
 int pick_bn(int N) {
-  static const int cand[] = {256, 224, 192, 160, 128, 96, 64, 32};
+  static const int cand[] = {128, 96, 64, 32};   // MAX_BN = 128
   for (int bn : cand)
     if (N % bn == 0) return bn;
   return 0;
@@ -190,7 +190,7 @@ int launch(Params p, cudaStream_t stream) {
   const bool a_mn = (p.a_smn == 1 && p.a_sk != 1), b_mn = (p.b_smn == 1 && p.b_sk != 1);
   if (p.BN == 0) p.BN = pick_bn(p.N);
   SM3_REQUIRE(p.BN >= 32 && p.BN <= MAX_BN && p.BN % 32 == 0 && p.N % p.BN == 0, SM3_ERR_UNSUPPORTED_SHAPE,
-              "gemm: N=%d has no tile width (multiple of 32 <= 256 dividing N)", p.N);
+              "gemm: N=%d has no tile width (multiple of 32 <= 128 dividing N)", p.N);
   SM3_REQUIRE(aligned16(p.A) && aligned16(p.B) && aligned16(p.D), SM3_ERR_INVALID_ARG, "gemm: pointers must be 16B aligned");
   if (!a_mn) SM3_REQUIRE(p.a_smn % 4 == 0 && p.K % 4 == 0, SM3_ERR_UNSUPPORTED_SHAPE, "gemm: K-major A needs K%%4==0, lda%%4==0");
   else       SM3_REQUIRE(p.a_sk % 4 == 0 && p.M % 8 == 0, SM3_ERR_UNSUPPORTED_SHAPE, "gemm: MN-major A needs M%%8==0, lda%%4==0");
@@ -229,7 +229,7 @@ int launch(Params p, cudaStream_t stream) {
     const long long b_ext = packed ? 0 : b_mn ? (long long)(p.b_k_index ? 1 : p.K) * p.b_sk + p.N : (long long)p.N * p.b_smn;
     SM3_REQUIRE(a_ext < (1LL << 32) && b_ext < (1LL << 32), SM3_ERR_UNSUPPORTED_SHAPE, "gemm: operand larger than 2^32 elements");
   }
-  // smem ring: 4 stages of 48 KB when a producer warp group writes the stage; fully packed operands only need
+  // smem ring: 6 stages of 32 KB when the producer warps write the stage; fully packed operands only need
   // 16 KB (A) + the two B planes per stage, so narrow tiles get a deeper ring (more bytes in flight per SM -- the
   // narrow GEMMs of stages 0/1 are HBM-bound streams of the packed A image).
   p.nstages = STAGES; p.stage_bytes = STAGE_BYTES;

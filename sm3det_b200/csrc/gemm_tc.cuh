@@ -1,48 +1,49 @@
-// Split-bf16 ("bf16x3") tensor-core GEMM for sm_100a: D[M,N] = epilogue( sum_k A(m,k) * B(n,k) ).
+// Split-bf16 ("bf16x3") tensor-core GEMM for sm_90a: D[M,N] = epilogue( sum_k A(m,k) * B(n,k) ).
 //
 // fp32 operands live in HBM.  Producer warps load them (coalesced float4, optional row gather),
 // split every value into bf16 hi + bf16 lo (a = hi + lo, |a-(hi+lo)| <= 2^-17 |a|), and store both
-// planes straight into the UMMA canonical shared-memory layouts (K-major SWIZZLE_64B or MN-major
-// SWIZZLE_128B).  One elected thread issues tcgen05.mma.kind::f16 three times per k-step
-// (hi*hi + hi*lo + lo*hi) into an fp32 accumulator in TMEM, so the product error is ~1e-5 relative
-// (vs 5e-4 for single-pass TF32) at 3 bf16 MMAs per logical MAC.  Epilogue warps read the
-// accumulator with tcgen05.ld and apply the fused epilogue (bias / GELU / GELU' / layer-scale /
-// gate / residual / atomic split-K).
+// planes straight into the wgmma canonical shared-memory layouts (K-major SWIZZLE_64B or MN-major
+// SWIZZLE_128B).  Two consumer warpgroups (64 rows of the 128-row tile each) issue wgmma.mma_async
+// three times per k-step (hi*hi + hi*lo + lo*hi) into fp32 register accumulators, so the product error
+// is ~1e-5 relative (vs 5e-4 for single-pass TF32) at 3 bf16 MMAs per logical MAC.  The same warps
+// then apply the fused epilogue (bias / GELU / GELU' / layer-scale / gate / residual / atomic split-K)
+// while the producers already fill the ring with the next tile.
 //
 // Replaces, on the reference hot path (convnext_moe.py): nn.Linear pointwise_conv1/2 + GELU
 // (:389-404), the per-expert Python loop (:244) incl. the gather x[_batch_index] (:265), and the
 // 2x2/s2 downsample convs (:549-558); and autograd's dgrad/wgrad GEMMs for all of them.
 #pragma once
+#include <type_traits>
 #include "common.cuh"
 
 namespace sm3 {
 namespace gemm {
 
-constexpr int BM = 128;          // UMMA M (rows of D per tile)
-constexpr int BK = 32;           // bf16 elements per k-block (2 UMMA k-steps of 16)
-constexpr int MAX_BN = 256;
-constexpr int STAGES = 4;
-constexpr int NUM_EPI_WARPS = 4;
-constexpr int MMA_WARP = 4;
-constexpr int NUM_PROD_WARPS = 7;
-constexpr int FIRST_PROD_WARP = 5;
-constexpr int NUM_THREADS = (NUM_EPI_WARPS + 1 + NUM_PROD_WARPS) * 32;  // 384 = 12 warps (register file is allocated in groups of 4 warps)
-constexpr int MAX_UNITS = 7;     // producer units per warp per k-block: ceil((128+256)/8 / 7)
+constexpr int BM = 128;          // rows of D per tile (two m64 warpgroup MMAs)
+constexpr int BK = 32;           // bf16 elements per k-block (2 wgmma k-steps of 16)
+constexpr int MAX_BN = 128;      // the accumulator of a 64 x 128 slab is 64 registers per consumer thread
+constexpr int STAGES = 6;
+constexpr int NUM_CONS_WARPS = 8;                                    // warps 0-7: two consumer warpgroups
+constexpr int NUM_PROD_WARPS = 8;
+constexpr int FIRST_PROD_WARP = 8;                                   // warps 8-15: producers
+constexpr int NUM_THREADS = (NUM_CONS_WARPS + NUM_PROD_WARPS) * 32;  // 512
+constexpr int CONS_REGS = 144, PROD_REGS = 112;                       // setmaxnreg split of the 64K-entry register file
+constexpr int MAX_UNITS = 4;     // producer units per warp per k-block: (128 + 128) / 8 / 8
 
 constexpr uint32_t OFF_A_HI = 0;
 constexpr uint32_t OFF_A_LO = 8192;
 constexpr uint32_t OFF_B_HI = 16384;
-constexpr uint32_t OFF_B_LO = 32768;
-constexpr uint32_t STAGE_BYTES = 49152;
+constexpr uint32_t OFF_B_LO = 24576;
+constexpr uint32_t STAGE_BYTES = 32768;
+constexpr uint32_t WG_A_BYTES = 4096;     // offset of rows 64..127 in an A plane (both layouts): the second warpgroup's slab
 constexpr int MAX_STAGES = 8;             // fully packed kernels use as many stages as fit (narrow tiles need less smem per stage)
 constexpr uint32_t BAR_BYTES = 256;
 constexpr int EPI_CW = 16;                                          // accumulator columns per epilogue pass
 constexpr uint32_t EPI_STAGE_ROW_FLOATS = EPI_CW + 4;               // + 4 pad: conflict-free 16-byte accesses
 constexpr uint32_t EPI_STAGE_BYTES = 32 * EPI_STAGE_ROW_FLOATS * 4;  // per epilogue warp
-constexpr int MAX_EPI_WARPS = 8;                                    // fully packed kernels: the idle producer warps 8-11 join
+constexpr int MAX_EPI_WARPS = 8;
 constexpr int COLSUM_SMEM_COLS = 3072;                              // EPI_COLSUM accumulates per CTA in smem when N fits
 constexpr uint32_t SMEM_BYTES = STAGES * STAGE_BYTES + BAR_BYTES + MAX_EPI_WARPS * EPI_STAGE_BYTES + COLSUM_SMEM_COLS * 4 + 1024;  // +1024 alignment slack
-constexpr uint32_t TMEM_COLS = 512;  // two 256-column fp32 accumulators
 
 enum Sched : int { SCHED_DENSE = 0, SCHED_GROUPED = 1, SCHED_SPLITK = 2 };
 
@@ -114,23 +115,20 @@ __host__ __device__ inline uint64_t make_smem_desc(uint32_t smem_addr, bool mn_m
   if (mn_major) {
     d |= (uint64_t)((MN_LBO_BYTES >> 4) & 0x3FFFu) << 16;
     d |= (uint64_t)((MN_SBO_BYTES >> 4) & 0x3FFFu) << 32;
-    d |= (uint64_t)2 << 61;  // SWIZZLE_128B
+    d |= (uint64_t)1 << 62;  // SWIZZLE_128B
   } else {
     d |= (uint64_t)1 << 16;  // LBO unused for swizzled K-major
     d |= (uint64_t)((K_SBO_BYTES >> 4) & 0x3FFFu) << 32;
-    d |= (uint64_t)4 << 61;  // SWIZZLE_64B
+    d |= (uint64_t)2 << 62;  // SWIZZLE_64B
   }
-  d |= (uint64_t)1 << 46;    // descriptor version (Blackwell)
   return d;
 }
-__host__ __device__ inline uint32_t make_instr_desc(int n, bool a_mn, bool b_mn) {
-  return (1u << 4)                       // D format f32
-       | (1u << 7) | (1u << 10)          // A, B format bf16
-       | ((a_mn ? 1u : 0u) << 15) | ((b_mn ? 1u : 0u) << 16)
-       | ((uint32_t)(n >> 3) << 17) | ((uint32_t)(BM >> 4) << 24);
-}
-
 #if defined(__CUDACC__) && defined(SM3_GEMM_KERNEL_IMPL)
+}  // namespace gemm
+}  // namespace sm3
+#include "wgmma.cuh"
+namespace sm3 {
+namespace gemm {
 // ---------------------------------------------------------------------------------------------
 // PTX wrappers
 __device__ __forceinline__ uint32_t smem_u32(const void* p) {
@@ -151,67 +149,18 @@ __device__ __forceinline__ bool mbar_try_wait(uint32_t bar, uint32_t parity) {
       : "=r"(ok) : "r"(bar), "r"(parity) : "memory");
   return ok != 0;
 }
-// Bounded wait: a pipeline bug traps (launch failure) instead of hanging the GPU box.
+// Bounded wait: a pipeline bug traps (launch failure) instead of hanging the GPU.  No printf here: a function call
+// between wgmma issue and wait would make ptxas serialise the asynchronous MMAs.
 __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
   if (mbar_try_wait(bar, parity)) return;
   const long long t0 = clock64();
   while (!mbar_try_wait(bar, parity)) {
-    if (clock64() - t0 > 20000000000LL) {  // ~10 s
-      printf("sm3 gemm: mbarrier timeout (block %d thread %d bar %u parity %u)\n", blockIdx.x,
-             threadIdx.x, bar, parity);
-      __trap();
-    }
+    if (clock64() - t0 > 20000000000LL) __trap();  // ~10 s
   }
 }
 __device__ __forceinline__ void fence_proxy_async_smem() {
   asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
 }
-__device__ __forceinline__ void tc_fence_before() {
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-}
-__device__ __forceinline__ void tc_fence_after() {
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-}
-__device__ __forceinline__ void tc_commit(uint32_t bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];"
-               ::"r"(bar) : "memory");
-}
-__device__ __forceinline__ void tc_mma(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc,
-                                       uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate) : "memory");
-}
-__device__ __forceinline__ void tc_ld32(uint32_t taddr, float (&v)[32]) {
-  uint32_t r[32];
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]),
-        "=r"(r[7]), "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]),
-        "=r"(r[14]), "=r"(r[15]), "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]),
-        "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]),
-        "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr) : "memory");
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-#pragma unroll
-  for (int i = 0; i < 32; ++i) v[i] = __uint_as_float(r[i]);
-}
-
-// asynchronous TMEM load of 16 accumulator columns (one row per lane); the registers are valid after tc_wait_ld()
-__device__ __forceinline__ void tc_ld16_issue(uint32_t taddr, uint32_t (&r)[16]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-        "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr) : "memory");
-}
-__device__ __forceinline__ void tc_wait_ld() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-
 // ---------------------------------------------------------------------------------------------
 struct Tile {
   int m0, n0, group, k_begin, k_end;
@@ -265,67 +214,49 @@ __device__ __forceinline__ void split4(const float4& x, uint32_t& h01, uint32_t&
 }
 
 // ---------------------------------------------------------------------------------------------
-// Kernel.  Warp roles: 0-3 epilogue (TMEM lane quarters), 4 MMA issuer (one elected lane),
-// 5-11 producers.  A k-block of an operand is cut into "units" of 8 rows x 32 k (K-major) or
-// 2 k-rows x 128 mn (MN-major); unit u of a k-block belongs to producer warp u % 7.  All per-tile
-// address arithmetic is hoisted: a thread keeps one 32-bit element offset per (unit, half) and
+// Kernel.  Warp roles: 0-7 consumers (warpgroup g = warp / 4 owns rows 64g..64g+63 of the tile: wgmma main loop,
+// then the epilogue straight from its register accumulator), 8-15 producers.  A k-block of an operand is cut into
+// "units" of 8 rows x 32 k (K-major) or 2 k-rows x 128 mn (MN-major); unit u of a k-block belongs to producer warp
+// u % 8.  All per-tile address arithmetic is hoisted: a thread keeps one 32-bit element offset per (unit, half) and
 // advances it by a constant per k-block.
-// EPI_T >= 0: the epilogue flag set is a compile-time constant (the hot FFN / expert / wgrad variants: the epilogue warps
-// are the bottleneck of the HBM-bound GEMMs and spend a fifth of their issue slots resolving the runtime flag branches);
+// EPI_T >= 0: the epilogue flag set is a compile-time constant (the hot FFN / expert / wgrad variants: the epilogue
+// is on the critical path of the HBM-bound GEMMs and the runtime flag branches cost issue slots there);
 // EPI_T = -1: generic, flags read from Params.
 template <bool A_MN, bool B_MN, bool B_PACKED, bool A_PACKED, int EPI_T>
-__global__ void __maxnreg__(168) gemm_bf16x3_kernel(const __grid_constant__ Params p) {
+__global__ void __launch_bounds__(NUM_THREADS, 1) gemm_bf16x3_kernel(const __grid_constant__ Params p) {
   const int EPI = (EPI_T >= 0) ? EPI_T : p.epi;
   extern __shared__ uint8_t smem_raw[];
   const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
   const uint32_t bar_base = smem_base + STAGES * STAGE_BYTES;
   auto full_bar = [&](int s) { return bar_base + 8u * s; };
   auto empty_bar = [&](int s) { return bar_base + 64u + 8u * s; };
-  auto tfull_bar = [&](int a) { return bar_base + 128u + 8u * a; };
-  auto tempty_bar = [&](int a) { return bar_base + 144u + 8u * a; };
-  const uint32_t tmem_slot = bar_base + 160u;
   const int NST = p.nstages;
   const uint32_t STB = p.stage_bytes;
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
 
   if (threadIdx.x == 0) {
-    for (int s = 0; s < NST; ++s) { mbar_init(full_bar(s), A_PACKED ? 1 : NUM_PROD_WARPS + (B_PACKED ? 1 : 0)); mbar_init(empty_bar(s), 1); }
-    for (int a = 0; a < 2; ++a) { mbar_init(tfull_bar(a), 1); mbar_init(tempty_bar(a), A_PACKED ? MAX_EPI_WARPS : NUM_EPI_WARPS); }
+    for (int s = 0; s < NST; ++s) { mbar_init(full_bar(s), A_PACKED ? 1 : NUM_PROD_WARPS + (B_PACKED ? 1 : 0)); mbar_init(empty_bar(s), NUM_CONS_WARPS); }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  if (warp == MMA_WARP) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;"
-                 ::"r"(tmem_slot), "r"(TMEM_COLS) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  uint32_t tmem_base;
-  asm volatile("ld.shared.u32 %0, [%1];" : "=r"(tmem_base) : "r"(tmem_slot) : "memory");
 
   const int ntiles = total_tiles(p);
 
-  constexpr int NE = A_PACKED ? MAX_EPI_WARPS : NUM_EPI_WARPS;
-  if (warp < NUM_EPI_WARPS || (A_PACKED && warp >= 8)) {
-    // ============================== EPILOGUE ==============================================
-    // TMEM -> registers (lane = row) -> per-warp smem transpose -> (lane = 4 columns) so that every global
-    // access of the epilogue (stores, residual / saved-activation loads, atomics) is a coalesced 128-byte row.
-    int acc = 0; uint32_t acc_phase = 0;
+  if (warp < NUM_CONS_WARPS) {
+    asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(CONS_REGS));
+    // ============================== CONSUMERS: MMA + EPILOGUE ===============================
+    constexpr int NE = NUM_CONS_WARPS;
+    const int wg = warp >> 2;
     const int nchunks = p.BN / EPI_CW;
-    const int e_idx = (warp < NUM_EPI_WARPS) ? warp : warp - 4;       // 0..NE-1
-    const int quarter = warp & 3;                                      // TMEM lane quarter this warp may read
-    const int cgrp = e_idx >> 2, ncgrp = NE / 4;                       // column-chunk subset c = cgrp (mod ncgrp)
-    const int my_last = ((nchunks - 1 - cgrp) / ncgrp) * ncgrp + cgrp; // last chunk this warp reads
-    const uint32_t stage_base = bar_base + BAR_BYTES + (uint32_t)e_idx * EPI_STAGE_BYTES;
+    const uint32_t stage_base = bar_base + BAR_BYTES + (uint32_t)warp * EPI_STAGE_BYTES;
     const int rl = lane >> 2, c4 = (lane & 3) * 4;      // this lane's row-in-group-of-8 and first column of 4
     // EPI_COLSUM: column sums are accumulated per CTA in shared memory across all its tiles of one group and
     // flushed with one global atomic per column (instead of one per column per tile).
     const uint32_t cs_base = bar_base + BAR_BYTES + MAX_EPI_WARPS * EPI_STAGE_BYTES;
     const bool cs_smem = (EPI & EPI_COLSUM) && p.N <= COLSUM_SMEM_COLS;
     int cs_group = -1;
-    const int e_tid = e_idx * 32 + lane;
+    const int e_tid = warp * 32 + lane;
     auto epi_bar = []() { asm volatile("bar.sync 1, %0;" ::"n"(NE * 32) : "memory"); };
     auto cs_flush = [&](int group) {
       epi_bar();
@@ -342,49 +273,99 @@ __global__ void __maxnreg__(168) gemm_bf16x3_kernel(const __grid_constant__ Para
       epi_bar();
     };
     if (cs_smem) cs_flush(-1);
+    int stage = 0; uint32_t phase = 0;
+    constexpr uint32_t a_kstep = A_MN ? 2u * MN_SBO_BYTES : 32u;   // advance 16 k per wgmma
+    constexpr uint32_t b_kstep = B_MN ? 2u * MN_SBO_BYTES : 32u;
+    const uint32_t b_lo_off = B_PACKED ? OFF_B_HI + plane_bytes(p.BN, B_MN) : OFF_B_LO;   // packed: lo follows hi
+    float acc[MAX_BN / 2];
     for (int t = blockIdx.x; t < ntiles; t += gridDim.x) {
       const Tile tl = decode_tile(p, t);
-      if (tl.nkb() == 0) continue;
+      const int nkb = tl.nkb();
+      if (nkb == 0) continue;
       if (cs_smem && tl.group != cs_group) { if (cs_group >= 0) cs_flush(cs_group); cs_group = tl.group; }
-      const int row0 = tl.m0 + quarter * 32;
-      // residual (shortcut) rows are prefetched one chunk ahead -- and for the first chunk before the accumulator is even
-      // ready -- so the epilogue no longer stalls a full HBM round trip per 32x16 block (profiles/r01_ncu_gemm_ffn2_stage0_specialised.txt)
-      float4 rr[4], rn[4];
-      auto load_resid = [&](int c_, float4 (&dst)[4]) {
+      const int row0 = tl.m0 + wg * 64 + (warp & 3) * 16;
+      // residual (shortcut) rows of the first chunk are fetched before the main loop and the next chunk's while the
+      // current one is written out, so the epilogue does not stall a full HBM round trip per 16 x 16 block
+      float4 rr[2], rn[2];
+      auto load_resid = [&](int c_, float4 (&dst)[2]) {
         const int n_ = tl.n0 + c_ * EPI_CW + c4;
 #pragma unroll
-        for (int it = 0; it < 4; ++it) {
+        for (int it = 0; it < 2; ++it) {
           const int row = row0 + it * 8 + rl;
           dst[it] = (row < p.M) ? ldg_f4(p.resid + (long long)row * p.ld_resid + n_) : make_float4(0.f, 0.f, 0.f, 0.f);
         }
       };
-      if ((EPI & EPI_RESID) && cgrp < nchunks) load_resid(cgrp, rr);
-      mbar_wait(tfull_bar(acc), acc_phase);
-      tc_fence_after();
+      if (EPI & EPI_RESID) load_resid(0, rr);
+
+      // ---- main loop: one k-block's MMAs stay in flight while the previous stage is handed back to the producers.
+      // The wgmma shape (N = BN) is a template argument of the whole loop, so ptxas sees a single accumulator shape.
+      int prev = -1;
+      auto mainloop = [&](auto bn_c) {
+        constexpr int N = decltype(bn_c)::value;
+        for (int kb = 0; kb < nkb; ++kb) {
+          mbar_wait(full_bar(stage), phase);
+          wg::fence();
+          const uint32_t sb = smem_base + stage * STB + (uint32_t)wg * WG_A_BYTES;
+          const uint32_t sbb = smem_base + stage * STB;
+#pragma unroll
+          for (int j = 0; j < BK / 16; ++j) {
+            const uint64_t ahi = make_smem_desc(sb + OFF_A_HI + j * a_kstep, A_MN);
+            const uint64_t alo = make_smem_desc(sb + OFF_A_LO + j * a_kstep, A_MN);
+            const uint64_t bhi = make_smem_desc(sbb + OFF_B_HI + j * b_kstep, B_MN);
+            const uint64_t blo = make_smem_desc(sbb + b_lo_off + j * b_kstep, B_MN);
+            if (!(p.debug & 4)) {
+              const uint32_t accum = (kb > 0 || j > 0) ? 1u : 0u;
+              if (p.passes == 1) {
+                wg::mma<N, A_MN, B_MN>(acc, ahi, bhi, accum);
+              } else {
+                wg::mma<N, A_MN, B_MN>(acc, alo, bhi, accum);
+                wg::mma<N, A_MN, B_MN>(acc, ahi, blo, 1u);
+                wg::mma<N, A_MN, B_MN>(acc, ahi, bhi, 1u);
+              }
+            }
+          }
+          wg::commit();
+          if (prev >= 0) {
+            wg::wait<1>();
+            __syncwarp();
+            if (lane == 0) mbar_arrive(empty_bar(prev));
+          }
+          prev = stage;
+          if (++stage == NST) { stage = 0; phase ^= 1u; }
+        }
+      };
+      switch (p.BN) {
+        case 32: mainloop(std::integral_constant<int, 32>{}); break;
+        case 64: mainloop(std::integral_constant<int, 64>{}); break;
+        case 96: mainloop(std::integral_constant<int, 96>{}); break;
+        default: mainloop(std::integral_constant<int, 128>{}); break;
+      }
+      wg::wait<0>();
+      wg::fence_operand(acc);
+      __syncwarp();
+      if (lane == 0) mbar_arrive(empty_bar(prev));
+      if (p.debug & 4) {
+#pragma unroll
+        for (int i = 0; i < MAX_BN / 2; ++i) acc[i] = 0.f;
+      }
+
+      // ---- epilogue: registers (wgmma fragment: row 16w + lane/4 (+8), column pair 8q + 2(lane%4)) -> per-warp smem
+      // transpose -> (lane = 4 columns) so that every global access (stores, residual / saved-activation loads,
+      // atomics) is a coalesced row segment
       float* dbase = p.D + (long long)tl.group * p.d_group_stride;
       const float* bias = p.bias ? p.bias + (long long)tl.group * p.bias_group_stride : nullptr;
-      bool arrived = false;
-      uint32_t vr[EPI_CW];
-      const uint32_t tbase = tmem_base + ((uint32_t)(quarter * 32) << 16) + (uint32_t)(acc * 256);
-      if (cgrp < nchunks) tc_ld16_issue(tbase + (uint32_t)(cgrp * EPI_CW), vr);
-      for (int c = cgrp; c < nchunks; c += ncgrp) {
-        tc_wait_ld();
-        if (c == my_last) {
-          tc_fence_before();
-          __syncwarp();
-          if (lane == 0) mbar_arrive(tempty_bar(acc));
-          arrived = true;
-        }
+#pragma unroll
+      for (int c = 0; c < MAX_BN / EPI_CW; ++c) {
+        if (c >= nchunks) break;
         __syncwarp();                                     // previous chunk's reads of the stage are done
 #pragma unroll
-        for (int j = 0; j < EPI_CW / 4; ++j)
-          asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};"
-                       ::"r"(stage_base + (uint32_t)(lane * EPI_STAGE_ROW_FLOATS + 4 * j) * 4u),
-                         "r"(vr[4 * j]), "r"(vr[4 * j + 1]), "r"(vr[4 * j + 2]), "r"(vr[4 * j + 3]) : "memory");
-        if (c + ncgrp < nchunks) {
-          tc_ld16_issue(tbase + (uint32_t)((c + ncgrp) * EPI_CW), vr);   // in flight while this chunk is written out
-          if (EPI & EPI_RESID) load_resid(c + ncgrp, rn);
-        }
+        for (int qq = 0; qq < 2; ++qq)
+#pragma unroll
+          for (int h = 0; h < 2; ++h)
+            asm volatile("st.shared.v2.f32 [%0], {%1, %2};"
+                         ::"r"(stage_base + (uint32_t)((rl + 8 * h) * EPI_STAGE_ROW_FLOATS + 8 * qq + 2 * (lane & 3)) * 4u),
+                           "f"(acc[8 * c + 4 * qq + 2 * h]), "f"(acc[8 * c + 4 * qq + 2 * h + 1]) : "memory");
+        if ((EPI & EPI_RESID) && c + 1 < nchunks) load_resid(c + 1, rn);
         __syncwarp();
         const int n = tl.n0 + c * EPI_CW + c4;
         float4 bv = make_float4(0.f, 0.f, 0.f, 0.f), sv = make_float4(1.f, 1.f, 1.f, 1.f);
@@ -392,7 +373,7 @@ __global__ void __maxnreg__(168) gemm_bf16x3_kernel(const __grid_constant__ Para
         if (EPI & EPI_COLSCALE) sv = ldg_f4(p.col_scale + n);
         float4 cs = make_float4(0.f, 0.f, 0.f, 0.f);
 #pragma unroll
-        for (int it = 0; it < 4; ++it) {
+        for (int it = 0; it < 2; ++it) {
           const int r = it * 8 + rl;
           const int row = row0 + r;
           if (row >= p.M) continue;
@@ -421,7 +402,7 @@ __global__ void __maxnreg__(168) gemm_bf16x3_kernel(const __grid_constant__ Para
         }
         if (EPI & EPI_RESID) {
 #pragma unroll
-          for (int it = 0; it < 4; ++it) rr[it] = rn[it];
+          for (int it = 0; it < 2; ++it) rr[it] = rn[it];
         }
         if (EPI & EPI_COLSUM) {
           // lanes with the same (lane & 3) hold partial sums of the same 4 columns
@@ -444,59 +425,11 @@ __global__ void __maxnreg__(168) gemm_bf16x3_kernel(const __grid_constant__ Para
           }
         }
       }
-      if (!arrived) {               // this warp had no chunk in the tile (BN/16 < NE/4 never happens, but stay safe)
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(tempty_bar(acc));
-      }
-      acc ^= 1; if (acc == 0) acc_phase ^= 1;
     }
     if (cs_smem && cs_group >= 0) cs_flush(cs_group);
-  } else if (warp == MMA_WARP) {
-    // ============================== MMA ISSUER ============================================
-    if (lane == 0) {
-      const uint32_t idesc = make_instr_desc(p.BN, A_MN, B_MN);
-      int stage = 0; uint32_t phase = 0; int acc = 0; uint32_t acc_phase = 0;
-      constexpr uint32_t a_kstep = A_MN ? 2u * MN_SBO_BYTES : 32u;   // advance 16 k per UMMA
-      constexpr uint32_t b_kstep = B_MN ? 2u * MN_SBO_BYTES : 32u;
-      for (int t = blockIdx.x; t < ntiles; t += gridDim.x) {
-        const Tile tl = decode_tile(p, t);
-        const int nkb = tl.nkb();
-        if (nkb == 0) continue;
-        mbar_wait(tempty_bar(acc), acc_phase ^ 1u);
-        tc_fence_after();
-        const uint32_t tmem_d = tmem_base + (uint32_t)(acc * 256);
-        for (int kb = 0; kb < nkb; ++kb) {
-          mbar_wait(full_bar(stage), phase);
-          tc_fence_after();
-          const uint32_t sb = smem_base + stage * STB;
-#pragma unroll
-          for (int j = 0; j < BK / 16; ++j) {
-            const uint64_t ahi = make_smem_desc(sb + OFF_A_HI + j * a_kstep, A_MN);
-            const uint64_t alo = make_smem_desc(sb + OFF_A_LO + j * a_kstep, A_MN);
-            const uint32_t b_lo_off = B_PACKED ? OFF_B_HI + plane_bytes(p.BN, B_MN) : OFF_B_LO;   // packed: lo follows hi
-            const uint64_t bhi = make_smem_desc(sb + OFF_B_HI + j * b_kstep, B_MN);
-            const uint64_t blo = make_smem_desc(sb + b_lo_off + j * b_kstep, B_MN);
-            if (!(p.debug & 4)) {
-              const uint32_t accum = (kb > 0 || j > 0) ? 1u : 0u;
-              if (p.passes == 1) {
-                tc_mma(tmem_d, ahi, bhi, idesc, accum);
-              } else {
-                tc_mma(tmem_d, alo, bhi, idesc, accum);
-                tc_mma(tmem_d, ahi, blo, idesc, 1u);
-                tc_mma(tmem_d, ahi, bhi, idesc, 1u);
-              }
-            }
-          }
-          tc_commit(empty_bar(stage));
-          if (kb == nkb - 1) tc_commit(tfull_bar(acc));
-          if (++stage == NST) { stage = 0; phase ^= 1u; }
-        }
-        acc ^= 1; if (acc == 0) acc_phase ^= 1u;
-      }
-    }
   } else {
     // ============================== PRODUCERS =============================================
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(PROD_REGS));
     if (A_PACKED) {
       // Both operands are pre-split tile images: one thread streams them in with two cp.async.bulk per k-block.
       if (warp == FIRST_PROD_WARP && lane == 0) {
@@ -539,7 +472,7 @@ __global__ void __maxnreg__(168) gemm_bf16x3_kernel(const __grid_constant__ Para
     const uint32_t kr_lane = (uint32_t)lane >> 4, j_lane = (uint32_t)lane & 15u;
 
     // per-tile state
-    constexpr int MU = B_PACKED ? 3 : MAX_UNITS;   // units per producer warp per k-block
+    constexpr int MU = B_PACKED ? (16 + NUM_PROD_WARPS - 1) / NUM_PROD_WARPS : MAX_UNITS;   // units per producer warp per k-block
     uint32_t off[MU];               // element offset of this lane's chunk from the operand base (A) / group base (B)
     uint32_t vmask = 0;             // bit i: row / mn range valid
     const float* baseB = p.B;
@@ -722,13 +655,6 @@ __global__ void __maxnreg__(168) gemm_bf16x3_kernel(const __grid_constant__ Para
     }  // !A_PACKED
   }
 
-  tc_fence_before();
-  __syncthreads();
-  if (warp == MMA_WARP) {
-    tc_fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(TMEM_COLS)
-                 : "memory");
-  }
 }
 #endif  // __CUDACC__ && SM3_GEMM_KERNEL_IMPL
 

@@ -6,7 +6,7 @@
 //                       (Block.norm1/norm2 :369-374, OverlapPatchEmbed.norm :407-410), layer-scale + residual :388-395
 //   lsk_agg/squeeze/mix channel mean / max, conv_squeeze(2->2, 7x7) + sigmoid, weighted sum (LSKblock.forward :336-341)
 //   mul                 x * attn :343
-//   im2col / col2im     OverlapPatchEmbed.proj (7x7/s4 stem, 3x3/s2 downsamples) :405-406 lowered to the tcgen05 GEMM
+//   im2col / col2im     OverlapPatchEmbed.proj (7x7/s4 stem, 3x3/s2 downsamples) :405-406 lowered to the wgmma GEMM
 #include "common.cuh"
 #include "kernels.h"
 
@@ -43,7 +43,7 @@ __device__ __forceinline__ void dwg_load_tile(float* xs, const float* __restrict
   __syncthreads();
 }
 
-// lane = (row selector l/16, channel pair l%16); FFMA2 (fma.rn.f32x2) on channel pairs, as in stencil.cu's 7x7 kernel
+// lane = (row selector l/16, channel pair l%16); ffma2 on channel pairs, as in stencil.cu's 7x7 kernel
 template <int KS, int DIL>
 __global__ void __launch_bounds__(256) dwconv_tile_kernel(const float* __restrict__ x, const float* __restrict__ wt,
                                                          const float* __restrict__ bias, const float* __restrict__ resid,
@@ -77,7 +77,7 @@ __global__ void __launch_bounds__(256) dwconv_tile_kernel(const float* __restric
 #pragma unroll
       for (int j = 0; j < KS; ++j) {
         const int o = cc - j * DIL;
-        if (o >= 0 && o < GT) asm("fma.rn.f32x2 %0, %1, %2, %0;" : "+l"(acc[o]) : "l"(v), "l"(wv[j]));
+        if (o >= 0 && o < GT) acc[o] = ffma2(v, wv[j], acc[o]);
       }
     }
   }

@@ -50,7 +50,7 @@ __global__ void __launch_bounds__(256, 2) moe_router_kernel(const RouterArgs a, 
     for (int j = 0; j < PJ; ++j) acc2[i][j] = 0ull;
   // Staging is software-pipelined: the global loads of k-chunk i+1 (8 KB of tokens + P x 128 B of Wp per block) are in
   // flight in registers while chunk i is multiplied -- the un-pipelined version spent most of its time in `long
-  // scoreboard` at the staging stores (profiles/r01_ncu_router_before.txt).
+  // scoreboard` at the staging stores.
   constexpr int NLD = 2 + PJ;                      // float4 per thread per chunk: (RT + 32*PJ) rows x 8 float4 / 256 threads
   float4 pre[NLD];
   auto gload = [&](int k0) {
@@ -87,7 +87,7 @@ __global__ void __launch_bounds__(256, 2) moe_router_kernel(const RouterArgs a, 
     sstore();
     __syncthreads();
     if (k0 + R_KC < C) gload(k0 + R_KC);
-    // FFMA2 (fma.rn.f32x2 = two IEEE fp32 FMAs per lane per issue, bit-identical to fmaf): accumulators are token pairs
+    // accumulators are token pairs (ffma2: two IEEE fp32 FMAs on a 64-bit pair)
 #pragma unroll 4
     for (int kk = 0; kk < R_KC; ++kk) {
       unsigned long long av2[4], bv2[PJ];
@@ -102,7 +102,7 @@ __global__ void __launch_bounds__(256, 2) moe_router_kernel(const RouterArgs a, 
       for (int i = 0; i < 4; ++i)
 #pragma unroll
         for (int j = 0; j < PJ; ++j)
-          asm("fma.rn.f32x2 %0, %1, %2, %0;" : "+l"(acc2[i][j]) : "l"(av2[i]), "l"(bv2[j]));
+          acc2[i][j] = ffma2(av2[i], bv2[j], acc2[i][j]);
     }
   }
 #pragma unroll

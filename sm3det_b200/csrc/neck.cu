@@ -1,5 +1,5 @@
 // MultitaskFPN helpers (SURVEY.md 8(f) rank 1: the consumer of the backbone's 4-tuple).  The 1x1 lateral and 3x3 output
-// convolutions run on the tcgen05 GEMM through im2col (lsk.cu); this file holds the two remaining data-movement kernels:
+// convolutions run on the wgmma GEMM through im2col (lsk.cu); this file holds the two remaining data-movement kernels:
 //   upsample_add      laterals[i-1] + F.interpolate(laterals[i], size=prev_shape, mode='nearest')
 //                     (reference mmrotate/models/necks/Multitask_FPN.py:123-134) and its backward,
 //   transpose_batched NHWC <-> NCHW conversion of the returned pyramid levels (the reference is NCHW end to end).

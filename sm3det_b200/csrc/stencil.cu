@@ -101,14 +101,8 @@ __device__ __forceinline__ void dw_load_tile(float* xs, const float* __restrict_
   __syncthreads();
 }
 
-// Packed-FP32 helpers: Blackwell issues FFMA2 (two fp32 FMAs per lane per instruction), which doubles the FMA rate of
-// this issue-bound stencil.  A "pair" is two adjacent channels held in one 64-bit register.
-typedef unsigned long long f32x2_t;
-__device__ __forceinline__ f32x2_t ffma2(f32x2_t a, f32x2_t b, f32x2_t c) {
-  f32x2_t d;
-  asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(d) : "l"(a), "l"(b), "l"(c));
-  return d;
-}
+// Packed-FP32 helpers (ffma2 in common.cuh): a "pair" is two adjacent channels held in one 64-bit register, so every
+// 64-bit shared-memory load feeds two FMAs of this issue-bound stencil.
 __device__ __forceinline__ f32x2_t pack2(float lo, float hi) {
   return (f32x2_t)__float_as_uint(lo) | ((f32x2_t)__float_as_uint(hi) << 32);
 }
@@ -117,7 +111,7 @@ __device__ __forceinline__ float2 unpack2(f32x2_t v) {
 }
 
 // lane = (row selector l/16, channel pair l%16): a half-warp owns one output row of the 16x16 tile and two channels per
-// lane, so every LDS.64 / FFMA2 does the work of two of the scalar version's instructions.
+// lane, so every LDS.64 does the work of two of the scalar version's loads.
 __global__ void __launch_bounds__(256) dwconv7_tile_kernel(const float* __restrict__ x, const float* __restrict__ wt,
                                                           const float* __restrict__ bias, const float* __restrict__ resid,
                                                           float* __restrict__ y, int H, int W, int C, int tiles_w,
@@ -253,7 +247,7 @@ __global__ void __launch_bounds__(256) dwconv7_wgrad_tile_kernel(const float* __
   float* ds = smem + DTI * DTI * DCC;             // [DT][DT][DCC]
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   const int c0 = blockIdx.y * DCC;
-  const int cp = lane & 15, half = lane >> 4;           // channel pair, row selector (FFMA2: two channels per lane)
+  const int cp = lane & 15, half = lane >> 4;           // channel pair, row selector (two channels per lane)
   f32x2_t acc[49];
 #pragma unroll
   for (int i = 0; i < 49; ++i) acc[i] = 0ull;

@@ -158,11 +158,10 @@ def _block_front_bwd(dv, dout, x, u, stats, dww, lnw):
 
 @ops.captures_precision
 class DenseBlockFn(Function):
-    """Dense ConvNeXt block.  Narrow stages (ops.ffn_chunk: C <= 192) run the FFN forward as the fused tcgen05 kernel of
+    """Dense ConvNeXt block.  Narrow stages (ops.ffn_chunk: C <= 192) run the FFN forward as the fused wgmma kernel of
     csrc/ffn_fused.cu (GEMM1 -> GELU -> GEMM2 on chip; the hidden tensor is written once, as fp32 h, only when a backward
-    follows).  The backward is the GEMM sequence (dgrad2 -> act_pack -> wgrads / dgrad1): fused recompute kernels for it
-    were built and measured slower (narrow tcgen05 MMAs are paced by the 64-byte/clk operand fetch, not by N --
-    profiles/r02_mma_microbench.txt).  Wider stages keep GEMM -> act_pack -> GEMM."""
+    follows).  The backward is the GEMM sequence (dgrad2 -> act_pack -> wgrads / dgrad1).  Wider stages keep
+    GEMM -> act_pack -> GEMM."""
 
     @staticmethod
     def forward(ctx, x, dww, dwb, lnw, lnb, w1, b1, w2, b2, gamma, row_scale, eps, packs):

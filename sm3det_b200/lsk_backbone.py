@@ -362,7 +362,7 @@ class LSKNet_moe(BaseModule):
     @staticmethod
     def _check_input(x):
         if not x.is_cuda:
-            raise RuntimeError('sm3det_b200 backbones run on CUDA (sm_100a) only; there is no CPU path')
+            raise RuntimeError('sm3det_b200 backbones run on CUDA (sm_90a) only; there is no CPU path')
         if x.dim() != 4:
             raise ValueError(f'expected [N,C,H,W], got {tuple(x.shape)}')
 

@@ -273,7 +273,7 @@ class AxpyFn(Function):
 
 @ops.captures_precision
 class PatchEmbedFn(Function):
-    """Conv2d(ks, stride, padding=ks//2) as im2col + tcgen05 GEMM.  x: NCHW (network input) or NHWC; out NHWC."""
+    """Conv2d(ks, stride, padding=ks//2) as im2col + wgmma GEMM.  x: NCHW (network input) or NHWC; out NHWC."""
 
     @staticmethod
     def forward(ctx, x, w, b, stride, nchw):

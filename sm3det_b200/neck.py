@@ -4,7 +4,7 @@ Same class name, constructor kwargs, ``state_dict`` keys (``lateral_convs.{i}.co
 ``forward(inputs, start_level=None, add_extra_convs=None)`` contract as the reference
 (mmrotate/models/necks/Multitask_FPN.py:14-162): consumes the backbone's tuple of NCHW maps, returns a tuple of NCHW maps.
 Inside, everything is NHWC: the 1x1 laterals read the NCHW inputs through im2col, the top-down path is one fused
-nearest-upsample + add kernel per level, the 3x3 (stride 1 / 2) output convolutions are im2col + tcgen05 GEMM, and only the
+nearest-upsample + add kernel per level, the 3x3 (stride 1 / 2) output convolutions are im2col + wgmma GEMM, and only the
 returned levels are transposed back to NCHW.
 """
 import torch
@@ -123,7 +123,7 @@ class MultitaskFPN(BaseModule):
         if add_extra_convs is None:
             add_extra_convs = self.add_extra_convs
         if not inputs[0].is_cuda:
-            raise RuntimeError('sm3det_b200 MultitaskFPN runs on CUDA (sm_100a) only; there is no CPU path')
+            raise RuntimeError('sm3det_b200 MultitaskFPN runs on CUDA (sm_90a) only; there is no CPU path')
         laterals = [_conv(lc, inputs[i + start_level], True) for i, lc in enumerate(self.lateral_convs[start_level:])]   # NHWC
         used = len(laterals)
         for i in range(used - 1, 0, -1):

@@ -89,7 +89,7 @@ def _pi(t):
 
 
 def _pick_bn(n: int) -> int:
-    for bn in (256, 224, 192, 160, 128, 96, 64, 32):
+    for bn in (128, 96, 64, 32):
         if n % bn == 0:
             return bn
     raise ValueError(f'N={n} has no GEMM tile width (multiple of 32)')
@@ -254,8 +254,8 @@ def act_pack(h, *, rows, width, mode, da=None, want_k=False, mn_tile=0, want_f32
 
 
 # When is an extra pack pass (8 B/element of HBM traffic) cheaper than splitting the operand inside the GEMM?  The
-# in-kernel split is repeated for every tile column that re-reads the operand and is latency/issue bound
-# (profiles/r01_gemm_isolation.txt); the packed main loop runs at the tensor-pipe rate.  Thresholds from measurements.
+# in-kernel split is repeated for every tile column that re-reads the operand and is latency/issue bound; the packed
+# main loop runs at the tensor-pipe rate.
 import os as _os
 PACK_A_MIN_K = int(_os.environ.get('SM3_PACK_A_MIN_K', '96'))
 PACK_W_MIN_TILES = int(_os.environ.get('SM3_PACK_W_MIN_TILES', '2'))

@@ -222,7 +222,7 @@ int main(int argc, char** argv) {
     check(128, 96, false);
     check(640, 96, true);
     check(200, 96, true);       // ragged last tile
-    check(45000, 96, false);    // > 148 x 2 tiles: every CTA loops, all ring phases wrap
+    check(45000, 96, false);    // > 132 x 2 tiles: every CTA loops, all ring phases wrap
     check(512, 64, true);
     check(384, 128, true);
     check(384, 192, false);

@@ -1,5 +1,5 @@
-// Standalone GPU check of the split-bf16 tcgen05 GEMM against a double-precision CPU reference.
-// Build: nvcc -gencode arch=compute_100a,code=sm_100a -O3 -std=c++17 -I sm3det_b200/csrc \
+// Standalone GPU check of the split-bf16 wgmma GEMM against a double-precision CPU reference.
+// Build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 -std=c++17 -I sm3det_b200/csrc \
 //        tests/cuda/gemm_test.cu sm3det_b200/csrc/gemm_tc.cu sm3det_b200/csrc/common.cu -o build/gemm_test
 #include "gemm_tc.cuh"
 #include <cmath>

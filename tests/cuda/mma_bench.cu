@@ -1,100 +1,88 @@
-// Microbenchmark: cost of one tcgen05.mma.kind::f16 (M = 128, K = 16, bf16 operands in shared memory, fp32 accumulator
-// in TMEM) as a function of N, issued back to back by one thread into the same accumulator -- the regime of the fused FFN
-// kernels (N = 32..96).  Answers: is a narrow MMA paced by N/2 tensor cycles, or by a per-instruction floor (operand fetch)?
+// Microbenchmark: cost of one wgmma.mma_async m64nNk16 (bf16 operands in shared memory, fp32 register accumulator)
+// as a function of N, issued back to back by one warpgroup into the same accumulator -- the regime of the fused FFN
+// kernels (N = 32..96).  Answers: is a narrow MMA paced by N, or by a per-instruction floor (operand fetch)?
 // Build: make build/mma_bench     Run: build/mma_bench
 #define SM3_GEMM_KERNEL_IMPL
 #include "gemm_tc.cuh"
 #include <cstdio>
 #include <vector>
 
+using namespace sm3;
 using namespace sm3::gemm;
-
-__device__ __forceinline__ uint64_t desc_mn64(uint32_t addr, uint32_t lbo) {
-  uint64_t d = 0;
-  d |= (uint64_t)((addr >> 4) & 0x3FFFu);
-  d |= (uint64_t)((lbo >> 4) & 0x3FFFu) << 16;
-  d |= (uint64_t)((512u >> 4) & 0x3FFFu) << 32;
-  d |= (uint64_t)1 << 46;
-  d |= (uint64_t)4 << 61;
-  return d;
-}
 
 // mode 0: K-major x K-major, the 3-pass pattern (alo*bhi, ahi*blo, ahi*bhi) over `ksteps` k-steps per round
 // mode 1: same operands every time (single descriptor pair)
 // mode 2: MN-major x MN-major (the wgrad operands)
-__global__ void __launch_bounds__(128, 1) mma_bench_kernel(int N, int mode, int rounds, int ksteps, long long* out) {
+template <int N>
+__global__ void __launch_bounds__(128, 1) mma_bench_kernel(int mode, int rounds, int ksteps, long long* out) {
   extern __shared__ uint8_t smem_raw[];
   const uint32_t sb = (smem_u32(smem_raw) + 1023u) & ~1023u;
-  __shared__ uint64_t bar;
-  __shared__ uint32_t tmem_slot;
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   for (uint32_t i = threadIdx.x; i < 160 * 1024 / 16; i += blockDim.x)
     asm volatile("st.shared.v4.b32 [%0], {%1, %1, %1, %1};" ::"r"(sb + i * 16), "r"(0x3C003C00u) : "memory");
   fence_proxy_async_smem();
-  if (threadIdx.x == 0) { mbar_init(smem_u32(&bar), 1); asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
-  if (warp == 0) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(&tmem_slot)), "r"(512) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem = tmem_slot;
-  if (warp == 1 && lane == 0) {
-    const bool mn = mode == 2;
-    const uint32_t idesc = make_instr_desc(N, mn, mn);
-    const uint32_t a0 = sb, b0 = sb + 64 * 1024;
-    const uint64_t da = mn ? desc_mn64(a0, 16384u) : make_smem_desc(a0, false);
-    const uint64_t db = mn ? desc_mn64(b0, 16384u) : make_smem_desc(b0, false);
-    const uint64_t kstep = mn ? 64u : 2u, lo = 512u;
-    uint32_t phase = 0;
-    const long long t0 = clock64();
-    for (int r = 0; r < rounds; ++r) {
-      for (int ks = 0; ks < ksteps; ++ks) {
-        const int kb = (ks >> 1) % 3;           // wrap inside a 3 k-block operand (48 KB of A, <= 96 KB of B)
-        const uint64_t a = da + (uint64_t)(ks & 1) * kstep + (uint64_t)kb * 1024u, b = db + (uint64_t)(ks & 1) * kstep + (uint64_t)kb * (mn ? 1024u : (uint64_t)N * 8u);
-        if (mode == 1) {
-          tc_mma(tmem, da, db, idesc, 1u); tc_mma(tmem, da, db, idesc, 1u); tc_mma(tmem, da, db, idesc, 1u);
-        } else {
-          tc_mma(tmem, a + lo, b, idesc, (r | ks) ? 1u : 0u);
-          tc_mma(tmem, a, b + (mn ? lo : (uint64_t)N * 4u), idesc, 1u);
-          tc_mma(tmem, a, b, idesc, 1u);
-        }
+  float acc[N / 2];
+#pragma unroll
+  for (int i = 0; i < N / 2; ++i) acc[i] = 0.f;
+  const bool mn = mode == 2;
+  const uint32_t a0 = sb, b0 = sb + 64 * 1024;
+  const uint64_t da = make_smem_desc(a0, mn), db = make_smem_desc(b0, mn);
+  const uint64_t kstep = mn ? 128u : 2u, lo = 512u;
+  const long long t0 = clock64();
+  for (int r = 0; r < rounds; ++r) {
+    wg::fence();
+    for (int ks = 0; ks < ksteps; ++ks) {
+      const int kb = (ks >> 1) % 3;           // wrap inside a 3 k-block operand (48 KB of A, <= 96 KB of B)
+      const uint64_t a = da + (uint64_t)(ks & 1) * kstep + (uint64_t)kb * 1024u, b = db + (uint64_t)(ks & 1) * kstep + (uint64_t)kb * (mn ? 1024u : (uint64_t)N * 8u);
+      if (mode == 1) {
+        wg::mma<N, 0, 0>(acc, da, db, 1u); wg::mma<N, 0, 0>(acc, da, db, 1u); wg::mma<N, 0, 0>(acc, da, db, 1u);
+      } else if (mode == 0) {
+        wg::mma<N, 0, 0>(acc, a + lo, b, 1u);
+        wg::mma<N, 0, 0>(acc, a, b + (uint64_t)N * 4u, 1u);
+        wg::mma<N, 0, 0>(acc, a, b, 1u);
+      } else {
+        wg::mma<N, 1, 1>(acc, a + lo, b, 1u);
+        wg::mma<N, 1, 1>(acc, a, b + lo, 1u);
+        wg::mma<N, 1, 1>(acc, a, b, 1u);
       }
-      tc_commit(smem_u32(&bar));
-      mbar_wait(smem_u32(&bar), phase);
-      phase ^= 1u;
     }
-    const long long t1 = clock64();
-    if (blockIdx.x == 0) out[0] = t1 - t0;
+    wg::commit();
+    wg::wait<0>();
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 0) {
-    tc_fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem), "r"(512) : "memory");
-  }
+  wg::fence_operand(acc);
+  const long long t1 = clock64();
+  float s = 0.f;
+#pragma unroll
+  for (int i = 0; i < N / 2; ++i) s += acc[i];
+  if (blockIdx.x == 0 && threadIdx.x == 0) { out[0] = t1 - t0; out[1] = (long long)s; }
+}
+
+template <int N>
+static int run(int grid, int mode, int ksteps, long long* d) {
+  const int smem = 161 * 1024 + 1024;
+  cudaFuncSetAttribute(mma_bench_kernel<N>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
+  const int rounds = 400 / (ksteps / 6);
+  mma_bench_kernel<N><<<grid, 128, smem>>>(mode, rounds, ksteps, d);
+  cudaError_t e = cudaDeviceSynchronize();
+  if (e != cudaSuccess) { printf("CUDA error %s\n", cudaGetErrorString(e)); return 1; }
+  long long cyc[2]; cudaMemcpy(cyc, d, 16, cudaMemcpyDeviceToHost);
+  const double per = (double)cyc[0] / ((double)rounds * ksteps * 3);
+  printf("grid %3d mode %d N=%3d  %2d k-steps/commit: %7.1f cycles/MMA  round latency %.0f\n", grid, mode, N, ksteps, per,
+         (double)cyc[0] / rounds);
+  return 0;
 }
 
 int main() {
-  long long* d; cudaMalloc(&d, 8);
-  const int smem = 161 * 1024 + 1024;
-  cudaFuncSetAttribute(mma_bench_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
-  printf("mode 0 = K-major 3-pass pattern, 1 = one descriptor pair repeated, 2 = MN-major 3-pass pattern; cycles per MMA (M=128,K=16)\n");
-  for (int grid : {1, 148}) {
+  long long* d; cudaMalloc(&d, 16);
+  int sms = 0; cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, 0);
+  printf("mode 0 = K-major 3-pass pattern, 1 = one descriptor pair repeated, 2 = MN-major 3-pass pattern; cycles per MMA (M=64,K=16)\n");
+  for (int grid : {1, sms}) {
     for (int mode = 0; mode < 3; ++mode) {
-      for (int N : {32, 64, 96, 128, 192, 256}) {
-        if (mode == 2 && N > 128) continue;        // the MN-major test operand is 4 groups of 32 wide
-        for (int ksteps : {6, 48}) {
-          const int rounds = 400 / (ksteps / 6);
-          mma_bench_kernel<<<grid, 128, smem>>>(N, mode, rounds, ksteps, d);
-          cudaError_t e = cudaDeviceSynchronize();
-          if (e != cudaSuccess) { printf("CUDA error %s\n", cudaGetErrorString(e)); return 1; }
-          long long cyc; cudaMemcpy(&cyc, d, 8, cudaMemcpyDeviceToHost);
-          const double per = (double)cyc / ((double)rounds * ksteps * 3);
-          printf("grid %3d mode %d N=%3d  %2d k-steps/commit: %7.1f cycles/MMA  (floor N/2 = %d)  round latency %.0f\n", grid, mode, N, ksteps, per, N / 2,
-                 (double)cyc / rounds);
-        }
+      for (int ksteps : {6, 48}) {
+        int rc = run<32>(grid, mode, ksteps, d) | run<64>(grid, mode, ksteps, d) | run<96>(grid, mode, ksteps, d) |
+                 run<128>(grid, mode, ksteps, d);
+        if (mode != 2) rc |= run<192>(grid, mode, ksteps, d) | run<256>(grid, mode, ksteps, d);   // MN-major test operand: 128 wide
+        if (rc) return 1;
       }
     }
   }

@@ -4,7 +4,7 @@ Emulates, on the CPU oracle, what each tensor-core operand format does to the FF
 backbone (ConvNeXt-T, E8 k2, one 1024^2 image, trained-like weights) -- forward AND backward GEMMs -- while everything the
 CUDA path keeps in fp32 SIMT (router, LayerNorm, depthwise conv, combine) stays fp32:
 
-  tf32_trunc : operands truncated to 10 mantissa bits (what tcgen05.mma.kind::tf32 does to raw fp32 bits in smem)
+  tf32_trunc : operands truncated to 10 mantissa bits (what a tf32 tensor-core MMA does to raw fp32 bits in smem)
   tf32_rn    : operands rounded to nearest-even at 10 bits (needs an extra rounding pass by the producer)
   bf16       : one bf16 pass (round to nearest) -- the AMP recipe
   bf16x3     : hi = truncated bf16, lo = rounded bf16 residual, hi*hi + hi*lo + lo*hi -- what sm3_gemm ships
@@ -13,7 +13,7 @@ and reports, against the unmodified fp32 oracle: max-norm relative error of the 
 and the largest (k)-vs-(k+1) logit gap among the flipped tokens (a flip with a large gap is a real routing change, not a
 numerical tie), and the worst parameter-gradient error.  Test infrastructure: imports oracle/, never the product.
 
-    python tests/diag/precision_study.py [--size 1024] [--modes tf32_trunc,tf32_rn,bf16,bf16x3] > profiles/r02_precision_study.txt
+    python tests/diag/precision_study.py [--size 1024] [--modes tf32_trunc,tf32_rn,bf16,bf16x3]
 """
 import argparse
 import os

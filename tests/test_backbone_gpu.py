@@ -5,7 +5,7 @@ import os
 import pytest
 import torch
 
-from oracle.cases import CASES, make_noise
+from oracle.cases import CASES, load_golden, make_noise
 from oracle.convnext_moe_oracle import OracleConfig, backbone_forward, param_shapes
 from oracle.gen_golden import moe_token_counts
 from sm3det_b200.synth import make_images, make_state_dict
@@ -22,7 +22,7 @@ def test_matches_reference_golden(path):
     (flips must be numerical ties), then outputs / loss / pre-gamma MoE outputs / every gradient vs the teacher-forced
     oracle on all elements, plus the fixture values themselves when no token flipped.  No assertion is conditional on
     the number of flips (see parity_util)."""
-    gold = torch.load(path, weights_only=False)
+    gold = load_golden(path)
     errs = run_case(gold['kw'], gold['img'], gold['mode'], gold['weights'], gold=gold, datasets=gold.get('datasets'))
     print(os.path.basename(path), errs)
 

@@ -40,6 +40,9 @@ def test_backbone_refuses_cpu_input():
         net(torch.zeros(1, 3, 64, 64))
 
 
+LIVE = os.path.join(ROOT, 'tests', 'golden', 'live', 'reference.pt')   # the reference's layouts (`python -m oracle.gen_golden live`)
+
+
 @pytest.mark.parametrize('kw,multi', [
     (dict(arch='tiny'), True),
     (dict(arch='tiny', MoE_Block_inds=[[], [], [0, 2, 4, 6, 8], [0, 2]], num_experts=8, top_k=2), True),
@@ -47,24 +50,26 @@ def test_backbone_refuses_cpu_input():
     (dict(arch='base', MoE_Block_inds=[[], [0, 2], list(range(0, 27, 2)), [0, 2]], num_experts=8, top_k=2), True),
 ])
 def test_state_dict_layout_matches_reference(kw, multi):
-    from oracle import ref_shim
+    from oracle.cases import load_golden
     from oracle.convnext_moe_oracle import OracleConfig, param_shapes
+    from oracle.gen_golden import LAYOUT_CASES
     from sm3det_b200 import build_backbone
     name = 'ConvNeXt_moe_MultiInput' if multi else 'ConvNeXt_moe'
     with torch.device('meta'):
         net = build_backbone(dict(type=name, **kw))
     mine = {k: tuple(v.shape) for k, v in net.state_dict().items()}
     assert mine == param_shapes(OracleConfig(multi_input=multi, **kw))
-    if ref_shim.reference_available() and kw['arch'] == 'tiny':
-        ref = ref_shim.build_reference_backbone(name, **kw)      # the reference cannot be built on 'meta'
-        assert mine == {k: tuple(v.shape) for k, v in ref.state_dict().items()}
-        assert sorted(n for n, _ in net.named_parameters()) == sorted(n for n, _ in ref.named_parameters())
+    if kw['arch'] == 'tiny':                                  # the reference's layouts were stored for the tiny cases
+        case = next(c for c, (cls, ckw) in LAYOUT_CASES.items() if cls == name and ckw == kw)
+        ref = load_golden(LIVE)['layout'][case]
+        assert mine == ref['shapes']
+        assert sorted(n for n, _ in net.named_parameters()) == ref['params']
 
 
 def test_convnext_da_state_dict_and_shared_gate_weights():
     """ConvNeXt_DA_MultiInput (convnext_moe_DA.py): same keys, order and parameter names as the reference, including its quirk
     of ONE gate MLP registered under fc.0 / fc.1 / fc.2; the literal config dict of local_configs/main_DA_*.py builds."""
-    from oracle import ref_shim
+    from oracle.cases import load_golden
     from oracle.convnext_moe_oracle import OracleConfig, param_shapes
     from sm3det_b200 import build_backbone
     kw = dict(arch='tiny', drop_path_rate=0.1, datasets=None)
@@ -75,10 +80,9 @@ def test_convnext_da_state_dict_and_shared_gate_weights():
     assert da.fc[0] is da.fc[1] is da.fc[2]
     names = [n for n, _ in net.named_parameters()]
     assert 'stages.0.0.DA.fc.0.0.weight' in names and 'stages.0.0.DA.fc.1.0.weight' not in names      # de-duplicated like the reference
-    if ref_shim.reference_available():
-        ref = ref_shim.build_reference_backbone('ConvNeXt_DA_MultiInput', module='convnext_moe_DA', **kw)
-        assert list(net.state_dict()) == list(ref.state_dict())
-        assert names == [n for n, _ in ref.named_parameters()]
+    ref = load_golden(LIVE)['layout']['da_tiny']
+    assert list(net.state_dict()) == ref['keys']
+    assert names == ref['params']
     with pytest.raises(NotImplementedError):
         build_backbone(dict(type='ConvNeXt_DA_MultiInput', arch='tiny', datasets=['sar', 'rgb', 'ifr']))
 
@@ -199,8 +203,8 @@ def test_ep_expert_layout_host_plan():
 
 
 def test_bench_resolves_the_named_configs():
-    """bench.py: the global batch of the named config is kept at every N (strong scaling), each GPU's share is one pass unless
-    --micro-batch splits it, cfg4 turns expert parallelism on at N > 1, --batch switches to weak scaling."""
+    """bench.py: the global batch of the named config is kept at every N (strong scaling), each GPU's share runs in passes of
+    at most 16 images unless --micro-batch sets the split, cfg4 turns expert parallelism on at N > 1, --batch switches to weak scaling."""
     import argparse
     import importlib.util
     spec = importlib.util.spec_from_file_location('bench_mod', os.path.join(ROOT, 'bench.py'))
@@ -213,7 +217,7 @@ def test_bench_resolves_the_named_configs():
         return argparse.Namespace(**d)
     for world, per in ((1, 32), (2, 16), (4, 8), (8, 4)):
         c, p, micro, scaling, ep = bench.resolve(ns(), world)
-        assert (p, micro, scaling, ep) == (per, per, 'strong', False)
+        assert (p, micro, scaling, ep) == (per, min(per, 16), 'strong', False)
     assert bench.resolve(ns(micro_batch=8), 1)[1:3] == (32, 8)
     assert bench.resolve(ns(micro_batch=5), 1)[2] == 4                      # largest divisor of the share not above the request
     assert bench.resolve(ns(batch=8), 4)[1:4] == (8, 8, 'weak')

@@ -8,7 +8,7 @@ import pytest
 import torch
 import torch.nn.functional as F
 
-from oracle.cases import LSK_CASES, lsk_injections, upstream_grads
+from oracle.cases import LSK_CASES, load_golden, lsk_injections, upstream_grads
 from oracle.lsk_moe_oracle import LskConfig, lsk_backbone_forward, lsk_param_shapes
 from sm3det_b200.synth import make_images, make_state_dict
 from parity_util import GAP_TOL, MAX_FLIP_FRACTION, assert_flips_are_near_ties, flipped_tokens
@@ -174,7 +174,7 @@ def inject(net, cfg, noise, drops):
 
 @pytest.mark.parametrize('path', sorted(glob.glob(os.path.join(GOLD, 'lsk_*.pt')) + glob.glob(os.path.join(GOLD, 'van_*.pt'))), ids=lambda p: os.path.basename(p)[:-3])
 def test_lsk_backbone_matches_reference_golden(path):
-    gold = torch.load(path, weights_only=False)
+    gold = load_golden(path)
     cfg, sd, net = build(gold['kw'], unit=gold.get('unit', 'lsk'))
     n, h, w = gold['img']
     x = make_images(n, h, w, seed=1234).cuda()
@@ -210,9 +210,8 @@ def test_lsk_backbone_matches_reference_golden(path):
 
     # LSKblock's channel max (lsk_moe.py:337) is the second discrete selection on this path: at 10^4..10^5 tokens per level a few
     # tokens have their two largest channels closer than the 3e-5 forward error, and ONE flipped token moves the whole d(max) of
-    # that token (a 7x7x2-tap sum over all channels) to another channel -- percent-level changes in the conv1/conv2 gradients
-    # (profiles/r02_lsk_argmax_flips.txt).  The forced-oracle pass below follows the CUDA path's channel choice, counts the
-    # tokens where that differs from the oracle's own argmax and requires each of them to be a numerical tie.
+    # that token (a 7x7x2-tap sum over all channels) to another channel -- percent-level changes in the conv1/conv2 gradients.
+    # The forced-oracle pass below follows the CUDA path's channel choice, counts the tokens where that differs from the oracle's own argmax and requires each of them to be a numerical tie.
     amax_flips, arec = 0, []
     is_lsk = gold.get('unit', 'lsk') == 'lsk'
     if full or flips > 0:

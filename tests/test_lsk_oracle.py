@@ -1,5 +1,5 @@
 """CPU checks for the LSKNet-MoE family: oracle vs committed goldens (generated from the real reference by
-oracle/gen_golden.py), oracle vs the live reference when /root/reference is present, and the drop-in contract
+oracle/gen_golden.py), oracle vs the reference module's stored outputs (tests/golden/live), and the drop-in contract
 (state_dict keys / shapes, constructor kwargs) of the CUDA module -- no GPU compute."""
 import glob
 import os
@@ -7,12 +7,12 @@ import os
 import pytest
 import torch
 
-from oracle import ref_shim
-from oracle.cases import LSK_CASES, lsk_injections
+from oracle.cases import LSK_CASES, load_golden, lsk_injections
 from oracle.lsk_moe_oracle import LskConfig, lsk_backbone_forward, lsk_param_shapes
 from sm3det_b200.synth import make_images, make_state_dict
 
 GOLD = os.path.join(os.path.dirname(__file__), 'golden')
+LIVE = os.path.join(GOLD, 'live', 'reference.pt')
 
 
 def _inputs(gold):
@@ -24,7 +24,7 @@ def _inputs(gold):
 
 @pytest.mark.parametrize('path', sorted(glob.glob(os.path.join(GOLD, 'lsk_*.pt')) + glob.glob(os.path.join(GOLD, 'van_*.pt'))), ids=lambda p: os.path.basename(p)[:-3])
 def test_oracle_reproduces_reference_golden(path):
-    gold = torch.load(path, weights_only=False)
+    gold = load_golden(path)
     if gold['mode'] != 'eval' and gold['img'][1] >= 512 and not os.environ.get('SM3_SLOW_TESTS'):
         pytest.skip('full-size training fixture: re-checked by oracle/gen_golden.py (set SM3_SLOW_TESTS=1 to run here)')
     cfg, sd, x = _inputs(gold)
@@ -35,31 +35,28 @@ def test_oracle_reproduces_reference_golden(path):
         res = lsk_backbone_forward(sd, cfg, x, train=gold['mode'] != 'eval', noise=noise, drop_masks=drops, record=rec, bn_state=bn)
     outs, loss = res if 'gate_loss' in gold else (res, None)
     st = gold.get('stride', 1)
+    # bit-exact where the fixture was generated; 2e-6 relative tolerates another CPU's kernel selection (as test_oracle.py)
     for o, g in zip(outs, gold['outs']):
-        assert torch.equal(o[:, :, ::st, ::st], g)
+        torch.testing.assert_close(o[:, :, ::st, ::st], g, rtol=2e-6, atol=2e-6)
     if loss is not None:
-        assert torch.equal(loss, gold['gate_loss'])
+        torch.testing.assert_close(loss, gold['gate_loss'], rtol=2e-6, atol=1e-9)
     for r, g in zip(rec, gold['moe']):
         assert torch.equal(r['top_idx'].to(g['top_idx'].dtype), g['top_idx'])
     for k, v in gold.get('bn', {}).items():
-        assert torch.equal(bn[k], v), k
+        torch.testing.assert_close(bn[k], v, rtol=2e-6, atol=2e-6, msg=k)
 
 
-@pytest.mark.skipif(not ref_shim.reference_available(), reason='reference tree not mounted')
 def test_oracle_matches_live_reference_lsk():
+    ref = load_golden(LIVE)['lsk']
     spec = LSK_CASES['lsk_mini_moe_e4k2_eval']
     cfg = LskConfig(**spec['kw'])
-    mod = ref_shim.load_reference_module('lsk_moe')
-    torch.manual_seed(0)
-    net = mod.LSKNet_moe_MultiInput(norm_cfg=dict(type='SyncBN', requires_grad=True), **spec['kw'])
     sd = make_state_dict(lsk_param_shapes(cfg), 0, True)
-    net.load_state_dict(sd, strict=True)
-    net.eval()
-    x = make_images(*spec['img'], seed=5)
     with torch.no_grad():
-        ref, rl = net(x)
-        orc, ol = lsk_backbone_forward(sd, cfg, x, train=False)
-    assert all(torch.equal(a, b) for a, b in zip(ref, orc)) and torch.equal(rl, ol)
+        orc, ol = lsk_backbone_forward(sd, cfg, make_images(*spec['img'], seed=5), train=False)
+    assert len(ref['outs']) == len(orc)
+    for a, b in zip(ref['outs'], orc):  # generated bit-exact; 2e-6 relative tolerates a different CPU kernel selection
+        torch.testing.assert_close(b, a, rtol=2e-6, atol=2e-6)
+    torch.testing.assert_close(ol, ref['loss'], rtol=2e-6, atol=2e-6)
 
 
 def test_lsk_contract_state_dict_and_registry():
@@ -81,12 +78,9 @@ def test_lsk_contract_state_dict_and_registry():
     assert set(lsk_param_shapes(pc)) == set(plain.state_dict())
     with pytest.raises(RuntimeError):
         net(torch.zeros(1, 3, 64, 64))                    # CPU tensor: no fallback path
-    if ref_shim.reference_available():
-        mod = ref_shim.load_reference_module('lsk_moe')
-        ref = mod.LSKNet_moe_MultiInput(**kw)
-        assert set(ref.state_dict()) == set(sd)
-        up = {k: v for k, v in ref.state_dict().items()}
-        assert not net.load_state_dict(up, strict=True).missing_keys
+    ref = load_golden(LIVE)['layout']['lsk_s']                                # the reference's state_dict keys and shapes
+    assert sorted(sd) == ref['keys']
+    assert {k: tuple(v.shape) for k, v in sd.items()} == ref['shapes']
 
 
 def test_lsk_upcycle_dense_checkpoint():
@@ -147,9 +141,8 @@ def test_van_contract():
     shapes = lsk_param_shapes(LskConfig(spatial_unit='lka', **kw))
     sd = net.state_dict()
     assert set(shapes) == set(sd) and all(tuple(sd[k].shape) == tuple(v) for k, v in shapes.items())
-    if ref_shim.reference_available():
-        ref = ref_shim.load_reference_module('van_moe').VAN_moe_MultiInput(**kw)
-        assert set(ref.state_dict()) == set(sd)
+    ref = load_golden(LIVE)['layout']['van']
+    assert sorted(sd) == ref['keys'] and {k: tuple(v.shape) for k, v in sd.items()} == ref['shapes']
 
 
 def test_forced_channel_argmax_is_identity_on_own_choice():

@@ -1,18 +1,23 @@
-"""The CPU oracle against (a) the committed golden fixtures generated from the unmodified reference
-and (b) the live reference module when /root/reference is present (build container only)."""
+"""The CPU oracle against the committed golden fixtures generated from the unmodified reference: (a) the parity cases of
+oracle/gen_golden.py and (b) the reference modules' own outputs on small cases (tests/golden/live, `gen_golden live`)."""
 import glob
 import os
 
 import pytest
 import torch
 
-from oracle import ref_shim
-from oracle.cases import CASES, make_noise, summarize_grad, upstream_grads
+from oracle.cases import CASES, load_golden, make_noise, summarize_grad, upstream_grads
 from oracle.convnext_moe_oracle import OracleConfig, backbone_forward, param_shapes, tie_da_weights
 from oracle.gen_golden import moe_token_counts
 from sm3det_b200.synth import make_images, make_state_dict, state_dict_checksum
 
 GOLD = os.path.join(os.path.dirname(__file__), 'golden')
+LIVE = os.path.join(GOLD, 'live', 'reference.pt')
+
+
+def _close(a, b):
+    # generated bit-exact against the oracle; 2e-6 relative tolerates a different CPU kernel selection
+    torch.testing.assert_close(a, b, rtol=2e-6, atol=2e-6)
 
 
 def _run_oracle(gold, record):
@@ -43,7 +48,7 @@ def _run_oracle(gold, record):
 
 @pytest.mark.parametrize('path', sorted(p for p in glob.glob(os.path.join(GOLD, '*.pt')) if not os.path.basename(p).startswith(('lsk_', 'van_'))), ids=lambda p: os.path.basename(p)[:-3])
 def test_oracle_matches_reference_golden(path):
-    gold = torch.load(path, weights_only=False)
+    gold = load_golden(path)
     if gold['mode'] != 'eval' and gold['img'][1] >= 512 and not os.environ.get('SM3_SLOW_TESTS'):
         pytest.skip('full-size training fixture: re-checked by oracle/gen_golden.py (set SM3_SLOW_TESTS=1 to run here)')
     record = []
@@ -69,47 +74,39 @@ def test_oracle_matches_reference_golden(path):
         (sum((o * u).sum() for o, u in zip(outs, ups)) + (loss if has_loss else 0.0)).backward()
         for name, g in gold['grads'].items():
             s = summarize_grad(sd[name].grad)
+            # atol 1e-6: summation order of another CPU's kernels (measured 4.7e-7 on one host)
             if 'full' in g:
-                torch.testing.assert_close(s['full'], g['full'], rtol=1e-5, atol=1e-7)
+                torch.testing.assert_close(s['full'], g['full'], rtol=1e-5, atol=1e-6)
             else:
-                torch.testing.assert_close(s['sample'], g['sample'], rtol=1e-5, atol=1e-7)
+                torch.testing.assert_close(s['sample'], g['sample'], rtol=1e-5, atol=1e-6)
                 assert abs(s['l2'] - g['l2']) <= 1e-5 * (g['l2'] + 1e-12)
 
 
-@pytest.mark.skipif(not ref_shim.reference_available(), reason='/root/reference not mounted')
 @pytest.mark.parametrize('name', ['mini_moe_e4k2_eval', 'mini_moe_e8k3_eval'])
 def test_oracle_matches_live_reference(name):
-    spec = CASES[name]
-    kw = dict(spec['kw'])
-    cfg = OracleConfig(**kw)
-    net = ref_shim.build_reference_backbone('ConvNeXt_moe_MultiInput', seed=0, **kw)
+    """ConvNeXt_moe_MultiInput of the reference (eval forward, seed-3 weights, two 64^2 images) vs the oracle."""
+    ref = load_golden(LIVE)['convnext'][name]
+    cfg = OracleConfig(**dict(CASES[name]['kw']))
     sd = make_state_dict(param_shapes(cfg), 3, True)
-    net.load_state_dict(sd, strict=True)
-    net.eval()
-    x = make_images(2, 64, 64, seed=5)
     with torch.no_grad():
-        ref = net(x)
-        orc = backbone_forward(sd, cfg, x)
-    for a, b in zip(ref[0], orc[0]):
-        assert torch.equal(a, b)
-    assert torch.equal(ref[1], orc[1])
+        orc = backbone_forward(sd, cfg, make_images(2, 64, 64, seed=5))
+    assert len(ref['outs']) == len(orc[0])
+    for a, b in zip(ref['outs'], orc[0]):
+        _close(b, a)
+    _close(orc[1], ref['loss'])
 
 
-@pytest.mark.skipif(not ref_shim.reference_available(), reason='/root/reference not mounted')
 def test_plain_convnext_moe_class_matches():
     """ConvNeXt_moe (stem inside downsample_layers.0) -- convnext_moe.py:407-600."""
+    ref = load_golden(LIVE)['convnext_plain']
     kw = dict(arch=dict(depths=[1, 1, 2, 1], channels=[32, 64, 96, 128]), MoE_Block_inds=[[], [], [1], []],
               num_experts=4, top_k=2)
     cfg = OracleConfig(multi_input=False, **kw)
-    net = ref_shim.build_reference_backbone('ConvNeXt_moe', seed=0, **kw)
     shapes = param_shapes(cfg)
-    assert set(shapes) == set(net.state_dict())
+    assert sorted(shapes) == ref['keys']
     sd = make_state_dict(shapes, 1, True)
-    net.load_state_dict(sd, strict=True)
-    net.eval()
-    x = make_images(1, 64, 64, seed=2)
     with torch.no_grad():
-        ref = net(x)
-        orc = backbone_forward(sd, cfg, x)
-    for a, b in zip(ref[0], orc[0]):
-        assert torch.equal(a, b)
+        orc = backbone_forward(sd, cfg, make_images(1, 64, 64, seed=2))
+    assert len(ref['outs']) == len(orc[0])
+    for a, b in zip(ref['outs'], orc[0]):
+        _close(b, a)
