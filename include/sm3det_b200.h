@@ -170,6 +170,14 @@ int sm3_dwconv7_fwd(const float* x, const float* weight_t, const float* bias, co
                     int32_t N, int32_t H, int32_t W, int32_t C, void* stream);
 int sm3_dwconv7_wgrad(const float* x, const float* dy, float* dweight_t, float* dbias, int32_t N, int32_t H,
                       int32_t W, int32_t C, void* stream);
+/* Block front in one pass: u = dwconv7(x) + bias (taps as [49][C]) and the block LayerNorm of u (:347-351).  Each output is
+ * written only when its pointer is non-null: u [T,C], stats (mean, rstd) [T,2], v [T,C] and img, the K-major bf16 hi|lo
+ * operand image of sm3_layernorm_fwd_img (C <= 256; rows of the last 128-row tile beyond T are zero).  C is a multiple of
+ * 32, at most 1024.  Bit-identical to sm3_dwconv7_fwd followed by sm3_layernorm_fwd, or by sm3_layernorm_fwd_img when
+ * img is requested (v and stats then follow that kernel's reduction order). */
+int sm3_dwconv7_ln_fwd(const float* x, const float* weight_t, const float* bias, const float* ln_weight,
+                       const float* ln_bias, float* u, float* stats, float* v, uint16_t* img, int32_t N, int32_t H,
+                       int32_t W, int32_t C, float eps, void* stream);
 
 /* ---- MoE routing --------------------------------------------------------------------------------
  * sm3_moe_router : CosineTopKGate.forward :99-106 + noisy_top_k_gating :194-223 (+ _prob_in_top_k

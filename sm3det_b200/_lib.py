@@ -102,6 +102,8 @@ SIGNATURES = {
     'sm3_stem_wgrad': [_P, _P, _P, _P, _I32, _I32, _I32, _I32, _I32, _I32, _P],
     'sm3_dwconv7_fwd': [_P, _P, _P, _P, _P, _I32, _I32, _I32, _I32, _P],  # x, wt, bias, resid, y, N, H, W, C, stream
     'sm3_dwconv7_wgrad': [_P, _P, _P, _P, _I32, _I32, _I32, _I32, _P],
+    # x, wt, bias, ln_weight, ln_bias, u, stats, v, img, N, H, W, C, eps, stream
+    'sm3_dwconv7_ln_fwd': [_P, _P, _P, _P, _P, _P, _P, _P, _P, _I32, _I32, _I32, _I32, _F32, _P],
     'sm3_moe_router_bwd_finalize': [_P, _P, _P, _I32, _I32, _P],
     'sm3_moe_router_blocks': [_I32],
     'sm3_moe_router': [C.POINTER(RouterArgs), _P],

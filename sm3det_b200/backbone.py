@@ -148,6 +148,7 @@ class ConvNeXtBlock(nn.Module):
             raise NotImplementedError('sm3det_b200: layer_scale_init_value must be > 0 (gamma is fused in the epilogue)')
         self.gamma = nn.Parameter(layer_scale_init_value * torch.ones((in_channels)), requires_grad=True)
         self.drop_path_rate = float(drop_path_rate)
+        self.with_cp = False      # set by the backbone (ConvNeXt_moe.with_cp)
         self._packs = PackCache()
 
     def _apply(self, fn, recurse=True):      # .to() / .cuda() / .half(): cached images no longer describe the weights
@@ -180,6 +181,10 @@ class ConvNeXtBlock(nn.Module):
         eps = self.norm.eps
         dw = self.depthwise_conv
         grad = torch.is_grad_enabled()
+        # activation checkpointing whenever a backward can follow a training step.  The checkpointed Functions compute
+        # bit-identical values, so unlike the reference (which also requires x.requires_grad) the choice needs no more
+        # conditions; it only trades memory for the recompute
+        checkpoint = self.with_cp and grad and self.training
         pc = self._packs
         from . import ops
         if self.MoE_cfg is None:
@@ -196,6 +201,7 @@ class ConvNeXtBlock(nn.Module):
                 packs['w1_t'] = pc.get('w1', [w1], True)
             packs['grad'] = grad
             packs['shortcut'] = shortcut
+            packs['checkpoint'] = checkpoint
             out = Fn.DenseBlockFn.apply(x, dw.weight, dw.bias, self.norm.weight, self.norm.bias,
                                         w1, f.pointwise_conv1.bias, w2, f.pointwise_conv2.bias, self.gamma, rs, eps, packs)
             return out, None
@@ -233,6 +239,7 @@ class ConvNeXtBlock(nn.Module):
             packs['w2_t'] = pc.get('w2', w2s, True)
             packs['wp_t'] = pc.get('wp', [g.cosine_projector.weight], True)
         packs['shortcut'] = shortcut
+        packs['checkpoint'] = checkpoint
         out, loss = Fn.MoEBlockFn.apply(x, dw.weight, dw.bias, self.norm.weight, self.norm.bias, self.gamma,
                                         g.cosine_projector.weight, g.cosine_projector.bias, g.sim_matrix, g.temperature,
                                         m.w_noise, rs, noise, eps, E, m.k, record, packs, *ep)
@@ -325,7 +332,6 @@ class ConvNeXt_moe(BaseModule):
         self.num_experts = num_experts
         self.frozen_stages = frozen_stages
         self.gap_before_final_norm = gap_before_final_norm
-        self.with_cp = with_cp     # accepted and ignored: no activation checkpointing (split large batches into passes instead)
         self.stem_patch_size = stem_patch_size
         self.norm_eps = norm_cfg.get('eps', 1e-5)
 
@@ -354,8 +360,23 @@ class ConvNeXt_moe(BaseModule):
             self.stages.append(stage)
             if i in self.out_indices:
                 self.add_module(f'norm{i}', build_LayerNorm2d_layer(norm_cfg, channels))
+        # activation checkpointing (reference :374-375): every block keeps only its input and the weights (plus the O(T*k)
+        # routing of a MoE block) for backward and recomputes the rest there; outputs and routing do not change.  The
+        # expert-parallel MoE blocks (sm3det_b200.expert_parallel) do not checkpoint.
+        self.with_cp = with_cp
         self._init_like_reference()
         self._freeze_stages()
+
+    @property
+    def with_cp(self):
+        return self._with_cp
+
+    @with_cp.setter
+    def with_cp(self, value):
+        self._with_cp = bool(value)
+        for stage in self.stages:
+            for blk in stage:
+                blk.with_cp = self._with_cp
 
     def _init_like_reference(self):
         """The reference never runs init_cfg (init_weights() only supports 'Pretrained'); weights stay at

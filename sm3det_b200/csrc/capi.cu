@@ -106,6 +106,11 @@ int sm3_dwconv7_wgrad(const float* x, const float* dy, float* dwt, float* dbias,
                       int32_t C, void* stream) {
   return dwconv7_wgrad(x, dy, dwt, dbias, N, H, W, C, S(stream));
 }
+int sm3_dwconv7_ln_fwd(const float* x, const float* wt, const float* bias, const float* lnw, const float* lnb, float* u,
+                       float* stats, float* v, uint16_t* img, int32_t N, int32_t H, int32_t W, int32_t C, float eps,
+                       void* stream) {
+  return dwconv7_ln_fwd(x, wt, bias, lnw, lnb, u, stats, v, img, N, H, W, C, eps, S(stream));
+}
 
 int sm3_moe_router_blocks(int32_t T) { return router_blocks(T); }
 int sm3_moe_router(const sm3_router_args* a, void* stream) {

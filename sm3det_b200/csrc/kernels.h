@@ -30,6 +30,11 @@ int dwconv7_fwd(const float* x, const float* wt, const float* bias, const float*
 int dwconv7_wgrad(const float* x, const float* dy, float* dwt, float* dbias, int N, int H, int W, int C,
                   cudaStream_t stream);
 
+// front.cu ---------------------------------------------------------------------------------------
+// dwconv7 + bias + block LayerNorm in one pass; each of u / stats / v / img is written only when non-null
+int dwconv7_ln_fwd(const float* x, const float* wt, const float* bias, const float* lnw, const float* lnb, float* u,
+                   float* stats, float* v, unsigned short* img, int N, int H, int W, int C, float eps, cudaStream_t stream);
+
 // moe.cu -----------------------------------------------------------------------------------------
 struct RouterArgs {
   const float* v;        // [T,C] LN output

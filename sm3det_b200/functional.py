@@ -156,6 +156,28 @@ def _block_front_bwd(dv, dout, x, u, stats, dww, lnw):
     return dx, ddww, ddwb, dlnw, dlnb
 
 
+def _dense_ffn(x, v, v_img, b1, w1, w2, b2, gamma, row_scale, resid, packs, keep):
+    """FFN + layer scale (+ drop-path row scale, + shortcut) of the dense block -> (out [T,C], h, y2).  keep: also return
+    what the backward reads, the pre-activation h [T,4C] and the pre-gamma output y2 [T,C] (else both None)."""
+    N, H, W, C = x.shape
+    T = N * H * W
+    fused = packs.get('fused')
+    if fused is not None:
+        res = ops.ffn_fused_fwd(v_img, packs['w1_c'][0], packs['w2_n'][0], b1, b2, T=T, C=C, chunk=fused['fwd'],
+                                gamma=gamma, row_scale=row_scale, resid=resid, want_aux=keep, want_h=keep)
+        return res[0], (res[2] if keep else None), res[1]
+    # GEMM1 stores the pre-activation only; GELU runs in the HBM-bound act_pack kernel, which emits the result
+    # directly as GEMM2's pre-split A operand (fp32 `a` never exists)
+    h = ops.linear_fwd(v, w1, b1, packed=packs.get('w1'))
+    a_k, _, _ = ops.act_pack(h, rows=T, width=4 * C, mode=ops.ACT_GELU, want_k=True)
+    y2 = torch.empty((T, C), device=x.device, dtype=torch.float32) if keep else None
+    epi = (EPI_COLSCALE | (EPI_RESID if resid is not None else 0) | (EPI_ROWSCALE if row_scale is not None else 0)
+           | (EPI_AUXSTORE if keep else 0))
+    out = ops.linear_fwd(None, w2, b2, rows=T, a_packed=a_k, epilogue=epi, aux_out=y2, col_scale=gamma,
+                         row_scale=row_scale, resid=resid, packed=packs.get('w2'))
+    return out, (h if keep else None), y2
+
+
 @ops.captures_precision
 class DenseBlockFn(Function):
     """Dense ConvNeXt block.  Narrow stages (ops.ffn_chunk: C <= 192) run the FFN forward as the fused wgmma kernel of
@@ -174,35 +196,48 @@ class DenseBlockFn(Function):
         # packs['shortcut'] = False: return the branch gamma * ffn(...) alone (ConvNeXt_DA gates it before the shortcut add)
         ctx.shortcut = packs.get('shortcut', True)
         resid = x.view(T, C) if ctx.shortcut else None
+        # packs['checkpoint']: activation checkpointing -- keep only the block input and the weights; backward recomputes the
+        # front (one dwconv7+LN pass, bit-identical to the two kernels below) and the FFN forward before the shared backward
+        ctx.checkpoint = train and packs.get('checkpoint', False)
+        if ctx.checkpoint:
+            _, _, v, v_img = ops.dwconv7_ln(x, _taps(dww), dwb, lnw, lnb, eps, want_v=fused is None, want_img=fused is not None)
+            out, _, _ = _dense_ffn(x, v, v_img, b1, w1, w2, b2, gamma, row_scale, resid, packs, keep=False)
+            ctx.save_for_backward(x, dww, dwb, lnw, lnb, w1, b1, w2, b2, gamma, row_scale)
+            ctx.eps = eps
+            ctx.packs = packs
+            return out.view(N, H, W, C)
         if fused is not None:
             # LayerNorm writes the FFN's A-operand image directly (the separate split pass never exists); the fused kernel
             # keeps the hidden tensor on chip and, when a backward follows, stores the pre-activation h once for it
             u = ops.dwconv7(x, _taps(dww), dwb)
             v_img, v, stats = ops.layernorm_fwd_img(u, lnw, lnb, eps, tokens=T, C=C, save_stats=train, want_f32=train)
-            res = ops.ffn_fused_fwd(v_img, packs['w1_c'][0], packs['w2_n'][0], b1, b2, T=T, C=C, chunk=fused['fwd'],
-                                    gamma=gamma, row_scale=row_scale, resid=resid, want_aux=train, want_h=train)
-            if train:
-                ctx.save_for_backward(x, u, stats, v, res[2], res[1], dww, lnw, w1, w2, gamma, row_scale)
-                ctx.packs = packs
-            return res[0].view(N, H, W, C)
-        u, v, stats = _block_front(x, dww, dwb, lnw, lnb, eps, train)
-        # GEMM1 stores the pre-activation only; GELU runs in the HBM-bound act_pack kernel, which emits the result
-        # directly as GEMM2's pre-split A operand (fp32 `a` never exists)
-        h = ops.linear_fwd(v, w1, b1, packed=packs.get('w1'))
-        a_k, _, _ = ops.act_pack(h, rows=T, width=4 * C, mode=ops.ACT_GELU, want_k=True)
-        y2 = torch.empty((T, C), device=x.device, dtype=torch.float32) if train else None
-        epi = (EPI_COLSCALE | (EPI_RESID if resid is not None else 0) | (EPI_ROWSCALE if row_scale is not None else 0)
-               | (EPI_AUXSTORE if train else 0))
-        out = ops.linear_fwd(None, w2, b2, rows=T, a_packed=a_k, epilogue=epi, aux_out=y2, col_scale=gamma,
-                             row_scale=row_scale, resid=resid, packed=packs.get('w2'))
+        else:
+            u, v, stats = _block_front(x, dww, dwb, lnw, lnb, eps, train)
+            v_img = None
+        out, h, y2 = _dense_ffn(x, v, v_img, b1, w1, w2, b2, gamma, row_scale, resid, packs, keep=train)
         if train:
             ctx.save_for_backward(x, u, stats, v, h, y2, dww, lnw, w1, w2, gamma, row_scale)
             ctx.packs = packs
         return out.view(N, H, W, C)
 
     @staticmethod
+    def _recompute(ctx, x, dww, dwb, lnw, lnb, w1, b1, w2, b2, gamma, rs):
+        """Checkpointed backward: rebuild (u, stats, v, h, y2) with the forward's own kernels and arguments."""
+        N, H, W, C = x.shape
+        want_img = ctx.packs.get('fused') is not None        # the plain forward's v and stats then come from layernorm_fwd_img
+        u, stats, v, v_img = ops.dwconv7_ln(x, _taps(dww), dwb, lnw, lnb, ctx.eps, want_u=True, want_stats=True, want_v=True,
+                                            want_img=want_img)
+        resid = x.view(N * H * W, C) if ctx.shortcut else None
+        _, h, y2 = _dense_ffn(x, v, v_img, b1, w1, w2, b2, gamma, rs, resid, ctx.packs, keep=True)
+        return u, stats, v, h, y2
+
+    @staticmethod
     def backward(ctx, dout):
-        x, u, stats, v, h, y2, dww, lnw, w1, w2, gamma, rs = ctx.saved_tensors
+        if ctx.checkpoint:
+            x, dww, dwb, lnw, lnb, w1, b1, w2, b2, gamma, rs = ctx.saved_tensors
+            u, stats, v, h, y2 = DenseBlockFn._recompute(ctx, x, dww, dwb, lnw, lnb, w1, b1, w2, b2, gamma, rs)
+        else:
+            x, u, stats, v, h, y2, dww, lnw, w1, w2, gamma, rs = ctx.saved_tensors
         N, H, W, C = x.shape
         T = N * H * W
         dout = dout.contiguous()
@@ -252,6 +287,17 @@ def stack_expert_params(params):
             p.data = flat[i]
 
 
+def _moe_experts(v, pair_token, grouped, w1, b1, w2, b2, R, packs):
+    """Grouped expert FFN over the padded expert segments -> (h [R,4C] pre-activation, o [R,C] expert outputs)."""
+    C = v.shape[1]
+    h = ops.linear_fwd(v, w1, b1, row_index=pair_token, rows=R, grouped=grouped, w_group_stride=4 * C * C,
+                       bias_group_stride=4 * C, packed=packs.get('w1'))
+    a_k, _, _ = ops.act_pack(h, rows=R, width=4 * C, mode=ops.ACT_GELU, want_k=True, live_tiles=grouped[1])
+    o = ops.linear_fwd(None, w2, b2, rows=R, a_packed=a_k, grouped=grouped, w_group_stride=4 * C * C,
+                       bias_group_stride=C, packed=packs.get('w2'))
+    return h, o
+
+
 @ops.captures_precision
 class MoEBlockFn(Function):
     """x -> dwconv -> LN -> router/plan/assign -> grouped expert GEMMs -> combine (+gamma, +shortcut)."""
@@ -263,41 +309,61 @@ class MoEBlockFn(Function):
         T = N * H * W
         w1s, b1s, w2s, b2s = experts[0:E], experts[E:2 * E], experts[2 * E:3 * E], experts[3 * E:4 * E]
         train = any(ctx.needs_input_grad)
-        u, v, stats = _block_front(x, dww, dwb, lnw, lnb, eps, train)
-        r = ops.moe_router(v, wp, bp, sim, tau, T=T, Cc=C, E=E, k=k, w_noise=w_noise, noise=noise, save=train)
+        # packs['checkpoint']: keep the block input, the weights and the O(T*k) routing (incl. the noise drawn for it);
+        # backward recomputes v bit-identically, hence the same router outputs, and the expert GEMMs over the saved plan
+        ctx.checkpoint = train and packs.get('checkpoint', False)
+        if ctx.checkpoint:
+            _, _, v, _ = ops.dwconv7_ln(x, _taps(dww), dwb, lnw, lnb, eps, want_v=True)
+        else:
+            u, v, stats = _block_front(x, dww, dwb, lnw, lnb, eps, train)
+        r = ops.moe_router(v, wp, bp, sim, tau, T=T, Cc=C, E=E, k=k, w_noise=w_noise, noise=noise,
+                           save=train and not ctx.checkpoint)
         plan = ops.moe_plan(r['partials'], T=T, E=E, k=k)
         slot_of, pair_token = ops.moe_assign(r['top_idx'], plan, T=T, E=E, k=k)
         R = plan['max_rows']
         grouped = (plan['tile_group'], plan['num_m_tiles'])
-        h = ops.linear_fwd(v, w1s[0], b1s[0], row_index=pair_token, rows=R, grouped=grouped, w_group_stride=4 * C * C,
-                           bias_group_stride=4 * C, packed=packs.get('w1'))
-        a_k, _, _ = ops.act_pack(h, rows=R, width=4 * C, mode=ops.ACT_GELU, want_k=True, live_tiles=plan['num_m_tiles'])
-        o = ops.linear_fwd(None, w2s[0], b2s[0], rows=R, a_packed=a_k, grouped=grouped, w_group_stride=4 * C * C,
-                           bias_group_stride=C, packed=packs.get('w2'))
+        h, o = _moe_experts(v, pair_token, grouped, w1s[0], b1s[0], w2s[0], b2s[0], R, packs)
         ctx.shortcut = packs.get('shortcut', True)
         out, y = ops.moe_combine(o, slot_of, r['top_idx'], r['top_gate'], gamma, x.view(T, C) if ctx.shortcut else None,
                                  row_scale, T=T, Cc=C, k=k, want_y=record is not None)
         if record is not None:
             record.append(dict(v=v, top_idx=r['top_idx'], top_gate=r['top_gate'], importance=plan['importance'],
                                load=plan['load'], loss=plan['loss'], y=y, counts=plan['counts']))
-        if train:
-            ctx.noisy = noise is not None     # gates depend on w_noise whenever noise was added, also for k == E
+        ctx.noisy = noise is not None         # gates depend on w_noise whenever noise was added, also for k == E
+        ctx.E, ctx.k, ctx.R = E, k, R
+        ctx.has_noise_param = w_noise is not None
+        if ctx.checkpoint:
+            ctx.save_for_backward(x, dww, dwb, lnw, lnb, gamma, wp, bp, sim, tau, row_scale, r['top_idx'], r['top_gate'],
+                                  slot_of, pair_token, plan['importance'], plan['seg_begin'], plan['seg_end'],
+                                  plan['tile_group'], plan['num_m_tiles'], w1s[0], b1s[0], w2s[0], b2s[0], noise, plan['load'],
+                                  w_noise)
+            ctx.eps = eps
+            ctx.packs = packs
+        elif train:
             ctx.save_for_backward(x, u, stats, v, h, o, dww, lnw, gamma, wp, sim, tau, row_scale, r['top_idx'],
                                   r['top_gate'], r['logits'], r['p'], slot_of, pair_token, plan['importance'],
                                   plan['seg_begin'], plan['seg_end'], plan['tile_group'], plan['num_m_tiles'],
                                   w1s[0], w2s[0], noise, r['sigma'], r['top_vals'], r['top_idx_m'], plan['load'],
                                   w_noise)
-            ctx.E, ctx.k, ctx.R = E, k, R
             ctx.packs = packs
-            ctx.has_noise_param = w_noise is not None
         return out.view(N, H, W, C), plan['loss'].reshape(())
 
     @staticmethod
     def backward(ctx, dout, dloss):
-        (x, u, stats, v, h, o, dww, lnw, gamma, wp, sim, tau, rs, top_idx, top_gate, logits, p, slot_of, pair_token,
-         importance, seg_begin, seg_end, tile_group, num_m_tiles, w1, w2, noise, sigma, top_vals, top_idx_m, load,
-         w_noise) = ctx.saved_tensors
         E, k, R = ctx.E, ctx.k, ctx.R
+        if ctx.checkpoint:
+            (x, dww, dwb, lnw, lnb, gamma, wp, bp, sim, tau, rs, top_idx, top_gate, slot_of, pair_token, importance,
+             seg_begin, seg_end, tile_group, num_m_tiles, w1, b1, w2, b2, noise, load, w_noise) = ctx.saved_tensors
+            N, H, W, C = x.shape
+            u, stats, v, _ = ops.dwconv7_ln(x, _taps(dww), dwb, lnw, lnb, ctx.eps, want_u=True, want_stats=True, want_v=True)
+            # the router only rebuilds what its backward reads; routing and plan are the saved ones (never re-planned)
+            r = ops.moe_router(v, wp, bp, sim, tau, T=N * H * W, Cc=C, E=E, k=k, w_noise=w_noise, noise=noise, save=True)
+            logits, p, sigma, top_vals, top_idx_m = r['logits'], r['p'], r['sigma'], r['top_vals'], r['top_idx_m']
+            h, o = _moe_experts(v, pair_token, (tile_group, num_m_tiles), w1, b1, w2, b2, R, ctx.packs)
+        else:
+            (x, u, stats, v, h, o, dww, lnw, gamma, wp, sim, tau, rs, top_idx, top_gate, logits, p, slot_of, pair_token,
+             importance, seg_begin, seg_end, tile_group, num_m_tiles, w1, w2, noise, sigma, top_vals, top_idx_m, load,
+             w_noise) = ctx.saved_tensors
         N, H, W, C = x.shape
         T = N * H * W
         dev = x.device

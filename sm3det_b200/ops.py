@@ -406,6 +406,23 @@ def dwconv7(x, wt, bias=None, resid=None, out=None):
     return out
 
 
+def dwconv7_ln(x, wt, bias, lnw, lnb, eps, *, want_u=False, want_stats=False, want_v=False, want_img=False):
+    """Block front in one pass (sm3_dwconv7_ln_fwd): u = dwconv7(x) + bias and its LayerNorm v.  Returns (u, stats, v, img),
+    absent outputs None.  Bit-identical to dwconv7 -> layernorm_fwd, or -> layernorm_fwd_img when want_img."""
+    lib = _lib.load()
+    N, H, W, Cc = x.shape
+    T = N * H * W
+    dev = x.device
+    u = torch.empty((N, H, W, Cc), device=dev, dtype=torch.float32) if want_u else None
+    stats = torch.empty((T, 2), device=dev, dtype=torch.float32) if want_stats else None
+    v = torch.empty((T, Cc), device=dev, dtype=torch.float32) if want_v else None
+    img = torch.empty((lib.sm3_gemm_packed_act_elems(T, Cc, 0, 128),), device=dev, dtype=torch.int16) if want_img else None
+    _lib.check(lib.sm3_dwconv7_ln_fwd(_p(x), _p(wt), _p(bias), _p(lnw), _p(lnb), _p(u), _p(stats), _p(v),
+                                      None if img is None else img.data_ptr(), N, H, W, Cc, float(eps), _stream()),
+               'sm3_dwconv7_ln_fwd')
+    return u, stats, v, img
+
+
 def dwconv7_wgrad(x, dy, dwt, dbias):
     lib = _lib.load()
     N, H, W, Cc = x.shape
