@@ -1,7 +1,7 @@
 // Split-bf16 ("bf16x3") tensor-core GEMM for sm_90a: D[M,N] = epilogue( sum_k A(m,k) * B(n,k) ).
 //
 // fp32 operands live in HBM.  Producer warps load them (coalesced float4, optional row gather),
-// split every value into bf16 hi + bf16 lo (a = hi + lo, |a-(hi+lo)| <= 2^-17 |a|), and store both
+// split every value into bf16 hi + bf16 lo (a = hi + lo, |a-(hi+lo)| <= 2^-16 |a|), and store both
 // planes straight into the wgmma canonical shared-memory layouts (K-major SWIZZLE_64B or MN-major
 // SWIZZLE_128B).  Two consumer warpgroups (64 rows of the 128-row tile each) issue wgmma.mma_async
 // three times per k-step (hi*hi + hi*lo + lo*hi) into fp32 register accumulators, so the product error
@@ -75,7 +75,12 @@ struct Params {
   int m_tiles, n_tiles, k_splits, num_groups;
   const int* tile_group;        // GROUPED: group id per m tile
   const int* num_m_tiles_dev;   // GROUPED: device scalar
-  const int* seg_begin;         // SPLITK: per-group reduction range (device) or null => [0,K)
+  // SPLITK: per-group reduction range [seg_begin, seg_end) (device) or null => [0,K).  The fully packed path (a_packed)
+  // bulk-copies whole 32-row k-blocks starting at k_begin / 32 and multiplies all of them, so it requires
+  // seg_begin % 32 == 0 and the rows [seg_end, ceil32(seg_end)) zero in one of the two operand images; the other paths
+  // mask k < seg_end.  The MoE, LSK and expert-parallel wgrads meet it: segments start at multiples of 128 and the rows
+  // past each segment's end are zero in d_o / gathered -1 rows (tests/test_gemm_gpu.py).
+  const int* seg_begin;
   const int* seg_end;
   // epilogue
   float* D; long long ldd; long long d_group_stride;

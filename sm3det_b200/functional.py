@@ -180,7 +180,7 @@ def _dense_ffn(x, v, v_img, b1, w1, w2, b2, gamma, row_scale, resid, packs, keep
 
 @ops.captures_precision
 class DenseBlockFn(Function):
-    """Dense ConvNeXt block.  Narrow stages (ops.ffn_chunk: C <= 192) run the FFN forward as the fused wgmma kernel of
+    """Dense ConvNeXt block.  Narrow stages (ops.ffn_chunk > 0: C a multiple of 32 up to 224) run the FFN forward as the fused wgmma kernel of
     csrc/ffn_fused.cu (GEMM1 -> GELU -> GEMM2 on chip; the hidden tensor is written once, as fp32 h, only when a backward
     follows).  The backward is the GEMM sequence (dgrad2 -> act_pack -> wgrads / dgrad1).  Wider stages keep
     GEMM -> act_pack -> GEMM."""

@@ -322,7 +322,9 @@ def linear_wgrad(dy, x, dw, *, rows=None, x_row_index=None, row_scale=None, segs
     """dw[g][N,K] += dy[rows_g, N]^T @ x[rows_g, K]  (split-K with fp32 atomics; dw must be pre-zeroed).
 
     row_scale (optional, [N]) scales the rows of dw (e.g. layer-scale gamma folded into the epilogue).
-    segs = (seg_begin, seg_end) device int32 arrays selecting each group's row range.
+    segs = (seg_begin, seg_end) device int32 arrays selecting each group's row range.  When the operands are packed
+    (dy_packed / x_packed given, or chosen below) the kernel reads whole 32-row blocks: every seg_begin must be a
+    multiple of 32, and the rows [seg_end, ceil32(seg_end)) must be zero in dy or in x (gathered -1 rows are zero).
     """
     R = rows if rows is not None else dy.shape[0]
     N = dw.shape[-2]

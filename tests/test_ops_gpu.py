@@ -6,6 +6,8 @@ import pytest
 import torch
 import torch.nn.functional as F
 
+from gemm_ref import decode_k_image
+
 pytestmark = pytest.mark.gpu
 
 
@@ -314,20 +316,6 @@ def test_ep_plan_kernel_matches_host_plan(W, E, k):
         ctx.overflow.zero_()
         device_plan(ctx, allm.cuda(), tile_group.cuda(), num_tiles.cuda(), pair_token.cuda(), E, R_s, 128)
         assert int(ctx.overflow) == R_d or R_d <= 128
-
-
-def decode_k_image(img, T, C):
-    """fp32 [T,C] value (hi + lo) of a K-major bf16 hi|lo operand image (128-row tiles, 32-k blocks, SWIZZLE_64B)."""
-    img = img.cpu().view(torch.int16).numpy().view('uint16')
-    t = torch.arange(T).view(-1, 1)
-    c = torch.arange(C).view(1, -1)
-    rt, rr, kb, ch, e = t // 128, t % 128, c // 32, (c % 32) // 8, c % 8
-    off = (rt * (C // 32) + kb) * 16384 + (rr >> 3) * 512 + (rr & 7) * 64 + ((ch ^ ((rr >> 1) & 3)) << 4) + e * 2
-    idx = (off // 2).numpy()
-
-    def bf(a):
-        return torch.from_numpy((a.astype('uint32') << 16).view('float32').copy())
-    return bf(img[idx]) + bf(img[idx + 4096])
 
 
 @pytest.mark.parametrize('T,C', [(300, 96), (1024, 64), (129, 192), (5, 128), (256, 32)])
