@@ -15,6 +15,7 @@ import torch
 import torch.nn as nn
 
 from . import functional as Fn
+from .moe_routing import gating_noise
 from .registry import ROTATED_BACKBONES, BaseModule
 
 ARCH_SETTINGS = {
@@ -206,13 +207,7 @@ class ConvNeXtBlock(nn.Module):
                                         w1, f.pointwise_conv1.bias, w2, f.pointwise_conv2.bias, self.gamma, rs, eps, packs)
             return out, None
         m = self.ffn
-        noise = None
-        if m.noisy_gating and self.training:
-            noise = getattr(m, '_injected_noise', None)
-            if noise is None:
-                T = x.shape[0] * x.shape[1] * x.shape[2]
-                noise = torch.randn((T, m.num_experts), device=x.device, dtype=torch.float32)
-            noise = noise.to(x.device, torch.float32).contiguous()
+        noise = gating_noise(m, x.shape[0] * x.shape[1] * x.shape[2], x.device)
         g = m.w_gate
         ep = m.expert_params()
         E = m.num_experts

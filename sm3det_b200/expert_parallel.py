@@ -28,6 +28,7 @@ from torch.autograd import Function
 
 from . import functional as Fn
 from . import ops
+from .moe_routing import Routing, route, router_backward
 
 
 class EPContext:
@@ -210,47 +211,36 @@ class EPMoEBlockFn(Function):
         u = ops.dwconv7(x, Fn._taps(dww), dwb)
         v = B['v'].view(T, C)
         _, stats = ops.layernorm_fwd(u, lnw, lnb, eps, tokens=T, C=C, out=v, save_stats=train)
-        r = ops.moe_router(v, wp, bp, sim, tau, T=T, Cc=C, E=E, k=k, w_noise=w_noise, noise=noise, save=train)
-        plan = ops.moe_plan(r['partials'], T=T, E=E, k=k)
-        slot_of, pair_token = ops.moe_assign(r['top_idx'], plan, T=T, E=E, k=k)
-        R_s, cap = plan['max_rows'], B['cap']
-        B['pair'][:R_s].copy_(pair_token)
-        meta = torch.stack([plan['counts'], plan['seg_begin']]).contiguous()
+        rt = route(v, wp, bp, sim, tau, w_noise, noise, E, k, save=train)
+        R_s, cap = rt.rows, B['cap']
+        B['pair'][:R_s].copy_(rt.pair_token)
+        meta = torch.stack([rt.counts, rt.seg_begin]).contiguous()
         allm = torch.empty((Wn, 2, E), device=dev, dtype=torch.int32)
         dist.all_gather_into_tensor(allm, meta, group=ep.group)      # also orders "v / pair list written" before peer reads
-        P = device_plan(ep, allm, plan['tile_group'], plan['num_m_tiles'], pair_token, E, R_s, cap)   # no host sync
+        P = device_plan(ep, allm, rt.tile_group, rt.num_m_tiles, rt.pair_token, E, R_s, cap)   # no host sync
         grouped = (P['tile_group'], P['num_tiles'])
         # every expert-side kernel runs over the fixed `cap` row space; the live tile count / segments come from the device
         xr = ops.gather_rows_peer(B['v_ptrs'], P['src_rank'], P['src_slot'], rows=cap, Cc=C, token_lists=B['pair_ptrs'])
-        h = ops.linear_fwd(xr, w1s[own], b1s[own], rows=cap, grouped=grouped, w_group_stride=4 * C * C,
-                           bias_group_stride=4 * C, packed=packs.get('w1'))
-        a_k, _, _ = ops.act_pack(h, rows=cap, width=4 * C, mode=ops.ACT_GELU, want_k=True, live_tiles=P['num_tiles'])
-        ops.linear_fwd(None, w2s[own], b2s[own], rows=cap, a_packed=a_k, grouped=grouped, w_group_stride=4 * C * C,
-                       bias_group_stride=C, packed=packs.get('w2'), out=B['o'][:cap * C].view(cap, C))
+        h, _ = Fn._moe_experts(xr, None, grouped, w1s[own], b1s[own], w2s[own], b2s[own], cap, packs,
+                               out=B['o'][:cap * C].view(cap, C))
         ep.barrier()                                                 # every rank's expert outputs are complete
         o = ops.gather_rows_peer(B['o_ptrs'], P['comb_rank'], P['comb_row'], rows=R_s, Cc=C)
-        out, y = ops.moe_combine(o, slot_of, r['top_idx'], r['top_gate'], gamma, x.view(T, C), row_scale, T=T, Cc=C, k=k,
+        out, y = ops.moe_combine(o, rt.slot_of, rt.top_idx, rt.top_gate, gamma, x.view(T, C), row_scale, T=T, Cc=C, k=k,
                                  want_y=record is not None)
         if record is not None:
-            record.append(dict(v=v.clone(), top_idx=r['top_idx'], top_gate=r['top_gate'], importance=plan['importance'],
-                               load=plan['load'], loss=plan['loss'], y=y, counts=plan['counts']))
+            record.append(dict(v=v.clone(), y=y, **rt.record()))
         if train:
-            ctx.noisy = noise is not None     # gates depend on w_noise whenever noise was added, also for k == E
-            ctx.save_for_backward(x, u, stats, v.clone(), h, xr, o, dww, lnw, gamma, wp, sim, tau, row_scale, r['top_idx'],
-                                  r['top_gate'], r['logits'], r['p'], slot_of, plan['importance'], w1s[own], w2s[own], noise,
-                                  r['sigma'], r['top_vals'], r['top_idx_m'], plan['load'], w_noise)
+            rt.save(ctx, x, u, stats, v.clone(), h, xr, o, dww, lnw, gamma, row_scale, w1s[own], w2s[own], dispatch=False)
             ctx.P, ctx.B, ctx.ep = P, B, ep
-            ctx.E, ctx.k, ctx.R_s, ctx.own, ctx.E_loc = E, k, R_s, own, E_loc
+            ctx.own, ctx.E_loc = own, E_loc
             ctx.packs = packs
-            ctx.has_noise_param = w_noise is not None
-        return out.view(N, H, W_, C), plan['loss'].reshape(())
+        return out.view(N, H, W_, C), rt.loss.reshape(())
 
     @staticmethod
     def backward(ctx, dout, dloss):
-        (x, u, stats, v, h, xr, o, dww, lnw, gamma, wp, sim, tau, rs, top_idx, top_gate, logits, p, slot_of, importance,
-         w1, w2, noise, sigma, top_vals, top_idx_m, load, w_noise) = ctx.saved_tensors
+        (x, u, stats, v, h, xr, o, dww, lnw, gamma, rs, w1, w2), rt = Routing.load(ctx)
         P, B, ep = ctx.P, ctx.B, ctx.ep
-        E, k, R_s, own, E_loc = ctx.E, ctx.k, ctx.R_s, ctx.own, ctx.E_loc
+        E, k, R_s, own, E_loc = rt.E, rt.k, rt.rows, ctx.own, ctx.E_loc
         N, H, W_, C = x.shape
         T = N * H * W_
         dev = x.device
@@ -262,53 +252,17 @@ class EPMoEBlockFn(Function):
         # slot is written, padding slots are never read: the expert side gathers through its source lists)
         d_o = B['do'][:R_s * C].view(R_s, C)
         dgamma = torch.zeros((C,), device=dev, dtype=torch.float32)
-        dgate = ops.moe_combine_bwd(dz, o, slot_of, top_idx, top_gate, gamma, rs, d_o, dgamma, T=T, Cc=C, k=k)
+        dgate = ops.moe_combine_bwd(dz, o, rt.slot_of, rt.top_idx, rt.top_gate, gamma, rs, d_o, dgamma, T=T, Cc=C, k=k)
         ep.barrier()                                                 # every rank's d_o rows are complete
-        # gradients exist for the OWNED experts only (the others return None and stay out of the DDP buckets)
-        dw1s = torch.zeros((E_loc, 4 * C, C), device=dev, dtype=torch.float32)
-        db1s = torch.zeros((E_loc, 4 * C), device=dev, dtype=torch.float32)
-        dw2s = torch.zeros((E_loc, C, 4 * C), device=dev, dtype=torch.float32)
-        db2s = torch.zeros((E_loc, C), device=dev, dtype=torch.float32)
         dor = ops.gather_rows_peer(B['do_ptrs'], P['src_rank'], P['src_slot'], rows=cap, Cc=C)
-        da = ops.linear_dgrad(dor, w2, grouped=grouped, w_group_stride=4 * C * C, packed=ctx.packs.get('w2_t'))
-        # one pass over h: dh = da * gelu'(h) as dgrad1's / wgrad1's operands (+ db1) and a = gelu(h) as wgrad2's operand
-        dh_k, dh_mn, a_mn = ops.act_pack(h, rows=cap, width=4 * C, mode=ops.ACT_BWD, da=da, want_k=True, mn_tile=128,
-                                      mn_tile2=ops._pick_bn(4 * C), colsum=db1s, live_tiles=P['num_tiles'], tile_group=P['tile_group'])
-        del da
-        ops.linear_wgrad(dor, None, dw2s, rows=cap, segs=segs, num_groups=E_loc, x_packed=a_mn)
-        del a_mn
-        ops.colsum(dor, db2s, rows=cap, Cc=C, segs=segs, groups=E_loc)
-        ops.linear_wgrad(None, xr, dw1s, rows=cap, segs=segs, num_groups=E_loc, dy_packed=dh_mn)
-        dxp = B['dxp'][:cap * C].view(cap, C)
-        ops.linear_dgrad(None, w1, rows=cap, a_packed=dh_k, out=dxp, grouped=grouped, w_group_stride=4 * C * C,
-                         packed=ctx.packs.get('w1_t'))
+        # gradients exist for the OWNED experts only (the others return None and stay out of the DDP buckets)
+        _, dw1s, db1s, dw2s, db2s = Fn._moe_experts_bwd(dor, xr, h, None, grouped, segs, w1, w2, E_loc, ctx.packs,
+                                                        dx_out=B['dxp'][:cap * C].view(cap, C))
         ep.barrier()                                                 # every rank's d_x rows are complete
         dxp_l = ops.gather_rows_peer(B['dxp_ptrs'], P['comb_rank'], P['comb_row'], rows=R_s, Cc=C)
-        # router (local)
-        Pp = wp.shape[0]
-        dtau = torch.zeros((1,), device=dev, dtype=torch.float32)
-        dsim = torch.zeros((Pp, E), device=dev, dtype=torch.float32)
-        lscale = dloss.reshape(1).contiguous().float()
-        noisy = dict(noise=noise, sigma=sigma, top_vals=top_vals, top_idx_m=top_idx_m, load=load) if ctx.noisy else None
-        dp, dr = ops.moe_router_bwd(p, sim, tau, top_idx, top_gate, dgate, logits, importance, lscale, dsim, dtau, T=T, E=E,
-                                    k=k, noisy=noisy)
-        dwp = torch.zeros_like(wp)
-        ops.linear_wgrad(dp, v, dwp)
-        dbp = torch.zeros((Pp,), device=dev, dtype=torch.float32)
-        ops.colsum(dp, dbp, rows=T, Cc=Pp)
-        dv_r = ops.linear_dgrad(dp, wp, packed=ctx.packs.get('wp_t'))
-        dwn = None
-        if ctx.noisy:
-            wn_t = torch.zeros((32, C), device=dev, dtype=torch.float32)
-            wn_t[:E] = w_noise.t()
-            dwn_t = torch.zeros((32, C), device=dev, dtype=torch.float32)
-            ops.linear_wgrad(dr, v, dwn_t)
-            dwn = dwn_t[:E].t().contiguous()
-            dv_r = ops.linear_dgrad(dr, wn_t, epilogue=ops.EPI_RESID, resid=dv_r)
-        dv = ops.gather_sum(dxp_l, slot_of, dv_r, T=T, Cc=C, k=k)
+        dv_r, dwp, dbp, dsim, dtau, dwn = router_backward(rt, v, dgate, dloss, wp_t=ctx.packs.get('wp_t'))
+        dv = ops.gather_sum(dxp_l, rt.slot_of, dv_r, T=T, Cc=C, k=k)
         dx, ddww, ddwb, dlnw, dlnb = Fn._block_front_bwd(dv, dout, x, u, stats, dww, lnw)
-        if dwn is None and ctx.has_noise_param:
-            dwn = torch.zeros((C, E), device=dev, dtype=torch.float32)
         if ep.average_grads:                  # what DDP's mean over ranks does to every other gradient
             for t in (dw1s, db1s, dw2s, db2s):
                 t.mul_(1.0 / ep.world)

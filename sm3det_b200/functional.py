@@ -16,6 +16,7 @@ import torch
 from torch.autograd import Function
 
 from . import ops
+from .moe_routing import Routing, route, router_backward
 from .ops import (EPI_AUXSTORE, EPI_COLSCALE, EPI_DGELU, EPI_GELU, EPI_RESID, EPI_ROWSCALE, LN_NCHW, LN_NHWC, LN_PATCH2)
 
 
@@ -23,12 +24,12 @@ def _zeros_like_param(p):
     return torch.zeros(p.shape, device=p.device, dtype=torch.float32)
 
 
-def _taps(dww):            # [C,1,7,7] -> [49][C]
-    return dww.reshape(dww.shape[0], 49).t().contiguous()
+def _taps(w):              # depthwise weight [C,1,ks,ks] -> [ks*ks][C]
+    return w.reshape(w.shape[0], -1).t().contiguous()
 
 
-def _taps_flipped(dww):    # correlation taps for dgrad
-    return dww.flip(2, 3).reshape(dww.shape[0], 49).t().contiguous()
+def _taps_flipped(w):      # correlation taps for dgrad
+    return w.flip(2, 3).reshape(w.shape[0], -1).t().contiguous()
 
 
 @ops.captures_precision
@@ -287,15 +288,41 @@ def stack_expert_params(params):
             p.data = flat[i]
 
 
-def _moe_experts(v, pair_token, grouped, w1, b1, w2, b2, R, packs):
-    """Grouped expert FFN over the padded expert segments -> (h [R,4C] pre-activation, o [R,C] expert outputs)."""
+def _moe_experts(v, row_index, grouped, w1, b1, w2, b2, R, packs, out=None):
+    """Grouped expert FFN over the R rows of the padded expert segments -> (h [R,4C] pre-activation, o [R,C] expert
+    outputs, written into `out` when given).  Row r reads v[row_index[r]], or v[r] when row_index is None."""
     C = v.shape[1]
-    h = ops.linear_fwd(v, w1, b1, row_index=pair_token, rows=R, grouped=grouped, w_group_stride=4 * C * C,
+    h = ops.linear_fwd(v, w1, b1, row_index=row_index, rows=R, grouped=grouped, w_group_stride=4 * C * C,
                        bias_group_stride=4 * C, packed=packs.get('w1'))
     a_k, _, _ = ops.act_pack(h, rows=R, width=4 * C, mode=ops.ACT_GELU, want_k=True, live_tiles=grouped[1])
     o = ops.linear_fwd(None, w2, b2, rows=R, a_packed=a_k, grouped=grouped, w_group_stride=4 * C * C,
-                       bias_group_stride=C, packed=packs.get('w2'))
+                       bias_group_stride=C, packed=packs.get('w2'), out=out)
     return h, o
+
+
+def _moe_experts_bwd(d_o, v, h, row_index, grouped, segs, w1, w2, G, packs, dx_out=None):
+    """Backward of _moe_experts for G expert groups from the expert-output gradient d_o [R,C].
+    -> (dxp [R,C] expert-input gradient rows, written into `dx_out` when given, dw1s, db1s, dw2s, db2s)."""
+    R, C = d_o.shape
+    dev = d_o.device
+    da = ops.linear_dgrad(d_o, w2, grouped=grouped, w_group_stride=4 * C * C, packed=packs.get('w2_t'))
+    db1s = torch.zeros((G, 4 * C), device=dev, dtype=torch.float32)
+    # one pass over h: dh = da * gelu'(h) as dgrad1's / wgrad1's operands (+ db1) and a = gelu(h) as wgrad2's operand
+    dh_k, dh_mn, a_mn = ops.act_pack(h, rows=R, width=4 * C, mode=ops.ACT_BWD, da=da, want_k=True, mn_tile=128,
+                                      mn_tile2=ops._pick_bn(4 * C), colsum=db1s, live_tiles=grouped[1], tile_group=grouped[0])
+    del da
+    dw2s = torch.zeros((G, C, 4 * C), device=dev, dtype=torch.float32)
+    ops.linear_wgrad(d_o, None, dw2s, rows=R, segs=segs, num_groups=G, x_packed=a_mn)
+    del a_mn
+    db2s = torch.zeros((G, C), device=dev, dtype=torch.float32)
+    ops.colsum(d_o, db2s, rows=R, Cc=C, segs=segs, groups=G)
+    dw1s = torch.zeros((G, 4 * C, C), device=dev, dtype=torch.float32)
+    ops.linear_wgrad(None, v, dw1s, rows=R, x_row_index=row_index, segs=segs, num_groups=G, dy_packed=dh_mn)
+    # every row the combine backward reads (live slots) is written by the GEMM
+    dxp = torch.empty((R, C), device=dev, dtype=torch.float32) if dx_out is None else dx_out
+    ops.linear_dgrad(None, w1, rows=R, a_packed=dh_k, out=dxp, grouped=grouped, w_group_stride=4 * C * C,
+                     packed=packs.get('w1_t'))
+    return dxp, dw1s, db1s, dw2s, db2s
 
 
 @ops.captures_precision
@@ -316,108 +343,44 @@ class MoEBlockFn(Function):
             _, _, v, _ = ops.dwconv7_ln(x, _taps(dww), dwb, lnw, lnb, eps, want_v=True)
         else:
             u, v, stats = _block_front(x, dww, dwb, lnw, lnb, eps, train)
-        r = ops.moe_router(v, wp, bp, sim, tau, T=T, Cc=C, E=E, k=k, w_noise=w_noise, noise=noise,
-                           save=train and not ctx.checkpoint)
-        plan = ops.moe_plan(r['partials'], T=T, E=E, k=k)
-        slot_of, pair_token = ops.moe_assign(r['top_idx'], plan, T=T, E=E, k=k)
-        R = plan['max_rows']
-        grouped = (plan['tile_group'], plan['num_m_tiles'])
-        h, o = _moe_experts(v, pair_token, grouped, w1s[0], b1s[0], w2s[0], b2s[0], R, packs)
+        rt = route(v, wp, bp, sim, tau, w_noise, noise, E, k, save=train and not ctx.checkpoint)
+        h, o = _moe_experts(v, rt.pair_token, rt.grouped, w1s[0], b1s[0], w2s[0], b2s[0], rt.rows, packs)
         ctx.shortcut = packs.get('shortcut', True)
-        out, y = ops.moe_combine(o, slot_of, r['top_idx'], r['top_gate'], gamma, x.view(T, C) if ctx.shortcut else None,
+        out, y = ops.moe_combine(o, rt.slot_of, rt.top_idx, rt.top_gate, gamma, x.view(T, C) if ctx.shortcut else None,
                                  row_scale, T=T, Cc=C, k=k, want_y=record is not None)
         if record is not None:
-            record.append(dict(v=v, top_idx=r['top_idx'], top_gate=r['top_gate'], importance=plan['importance'],
-                               load=plan['load'], loss=plan['loss'], y=y, counts=plan['counts']))
-        ctx.noisy = noise is not None         # gates depend on w_noise whenever noise was added, also for k == E
-        ctx.E, ctx.k, ctx.R = E, k, R
-        ctx.has_noise_param = w_noise is not None
+            record.append(dict(v=v, y=y, **rt.record()))
         if ctx.checkpoint:
-            ctx.save_for_backward(x, dww, dwb, lnw, lnb, gamma, wp, bp, sim, tau, row_scale, r['top_idx'], r['top_gate'],
-                                  slot_of, pair_token, plan['importance'], plan['seg_begin'], plan['seg_end'],
-                                  plan['tile_group'], plan['num_m_tiles'], w1s[0], b1s[0], w2s[0], b2s[0], noise, plan['load'],
-                                  w_noise)
+            rt.save(ctx, x, dww, dwb, lnw, lnb, gamma, row_scale, w1s[0], b1s[0], w2s[0], b2s[0])
             ctx.eps = eps
-            ctx.packs = packs
         elif train:
-            ctx.save_for_backward(x, u, stats, v, h, o, dww, lnw, gamma, wp, sim, tau, row_scale, r['top_idx'],
-                                  r['top_gate'], r['logits'], r['p'], slot_of, pair_token, plan['importance'],
-                                  plan['seg_begin'], plan['seg_end'], plan['tile_group'], plan['num_m_tiles'],
-                                  w1s[0], w2s[0], noise, r['sigma'], r['top_vals'], r['top_idx_m'], plan['load'],
-                                  w_noise)
-            ctx.packs = packs
-        return out.view(N, H, W, C), plan['loss'].reshape(())
+            rt.save(ctx, x, u, stats, v, h, o, dww, lnw, gamma, row_scale, w1s[0], w2s[0])
+        ctx.packs = packs
+        return out.view(N, H, W, C), rt.loss.reshape(())
 
     @staticmethod
     def backward(ctx, dout, dloss):
-        E, k, R = ctx.E, ctx.k, ctx.R
         if ctx.checkpoint:
-            (x, dww, dwb, lnw, lnb, gamma, wp, bp, sim, tau, rs, top_idx, top_gate, slot_of, pair_token, importance,
-             seg_begin, seg_end, tile_group, num_m_tiles, w1, b1, w2, b2, noise, load, w_noise) = ctx.saved_tensors
-            N, H, W, C = x.shape
+            (x, dww, dwb, lnw, lnb, gamma, rs, w1, b1, w2, b2), rt = Routing.load(ctx)
             u, stats, v, _ = ops.dwconv7_ln(x, _taps(dww), dwb, lnw, lnb, ctx.eps, want_u=True, want_stats=True, want_v=True)
-            # the router only rebuilds what its backward reads; routing and plan are the saved ones (never re-planned)
-            r = ops.moe_router(v, wp, bp, sim, tau, T=N * H * W, Cc=C, E=E, k=k, w_noise=w_noise, noise=noise, save=True)
-            logits, p, sigma, top_vals, top_idx_m = r['logits'], r['p'], r['sigma'], r['top_vals'], r['top_idx_m']
-            h, o = _moe_experts(v, pair_token, (tile_group, num_m_tiles), w1, b1, w2, b2, R, ctx.packs)
+            rt.rerun_router(v)
+            h, o = _moe_experts(v, rt.pair_token, rt.grouped, w1, b1, w2, b2, rt.rows, ctx.packs)
         else:
-            (x, u, stats, v, h, o, dww, lnw, gamma, wp, sim, tau, rs, top_idx, top_gate, logits, p, slot_of, pair_token,
-             importance, seg_begin, seg_end, tile_group, num_m_tiles, w1, w2, noise, sigma, top_vals, top_idx_m, load,
-             w_noise) = ctx.saved_tensors
+            (x, u, stats, v, h, o, dww, lnw, gamma, rs, w1, w2), rt = Routing.load(ctx)
         N, H, W, C = x.shape
         T = N * H * W
+        E, k = rt.E, rt.k
         dev = x.device
         dout = dout.contiguous()
         dz = dout.view(T, C)
-        grouped = (tile_group, num_m_tiles)
-        segs = (seg_begin, seg_end)
         # combine / layer scale / shortcut
-        d_o = torch.zeros((R, C), device=dev, dtype=torch.float32)
+        d_o = torch.zeros((rt.rows, C), device=dev, dtype=torch.float32)
         dgamma = torch.zeros((C,), device=dev, dtype=torch.float32)
-        dgate = ops.moe_combine_bwd(dz, o, slot_of, top_idx, top_gate, gamma, rs, d_o, dgamma, T=T, Cc=C, k=k)
-        # experts (grouped over the padded expert segments)
-        da = ops.linear_dgrad(d_o, w2, grouped=grouped, w_group_stride=4 * C * C, packed=ctx.packs.get('w2_t'))
-        db1s = torch.zeros((E, 4 * C), device=dev, dtype=torch.float32)
-        # one pass over h: dh = da * gelu'(h) as dgrad1's / wgrad1's operands (+ db1) and a = gelu(h) as wgrad2's operand
-        dh_k, dh_mn, a_mn = ops.act_pack(h, rows=R, width=4 * C, mode=ops.ACT_BWD, da=da, want_k=True, mn_tile=128,
-                                      mn_tile2=ops._pick_bn(4 * C), colsum=db1s, live_tiles=num_m_tiles, tile_group=tile_group)
-        del da
-        dw2s = torch.zeros((E, C, 4 * C), device=dev, dtype=torch.float32)
-        ops.linear_wgrad(d_o, None, dw2s, rows=R, segs=segs, num_groups=E, x_packed=a_mn)
-        del a_mn
-        db2s = torch.zeros((E, C), device=dev, dtype=torch.float32)
-        ops.colsum(d_o, db2s, rows=R, Cc=C, segs=segs, groups=E)
-        dw1s = torch.zeros((E, 4 * C, C), device=dev, dtype=torch.float32)
-        ops.linear_wgrad(None, v, dw1s, rows=R, x_row_index=pair_token, segs=segs, num_groups=E, dy_packed=dh_mn)
-        dxp = torch.empty((R, C), device=dev, dtype=torch.float32)   # every row gather_sum reads (live slots) is written by the GEMM
-        ops.linear_dgrad(None, w1, rows=R, a_packed=dh_k, out=dxp, grouped=grouped, w_group_stride=4 * C * C,
-                         packed=ctx.packs.get('w1_t'))
-        # router
-        P = wp.shape[0]
-        dtau = torch.zeros((1,), device=dev, dtype=torch.float32)
-        dsim = torch.zeros((P, E), device=dev, dtype=torch.float32)
-        lscale = dloss.reshape(1).contiguous().float()
-        noisy = dict(noise=noise, sigma=sigma, top_vals=top_vals, top_idx_m=top_idx_m, load=load) if ctx.noisy else None
-        dp, dr = ops.moe_router_bwd(p, sim, tau, top_idx, top_gate, dgate, logits, importance, lscale, dsim, dtau, T=T,
-                                    E=E, k=k, noisy=noisy)
-        dwp = torch.zeros_like(wp)
-        ops.linear_wgrad(dp, v, dwp)
-        dbp = torch.zeros((P,), device=dev, dtype=torch.float32)
-        ops.colsum(dp, dbp, rows=T, Cc=P)
-        dv_r = ops.linear_dgrad(dp, wp, packed=ctx.packs.get('wp_t'))
-        dwn = None
-        if ctx.noisy:
-            # r = v @ w_noise is an [T,C]x[C,E] product with E < 32: run it as a 32-wide zero-padded GEMM pair
-            wn_t = torch.zeros((32, C), device=dev, dtype=torch.float32)
-            wn_t[:E] = w_noise.t()
-            dwn_t = torch.zeros((32, C), device=dev, dtype=torch.float32)
-            ops.linear_wgrad(dr, v, dwn_t)                             # [32,C] = dr^T v
-            dwn = dwn_t[:E].t().contiguous()
-            dv_r = ops.linear_dgrad(dr, wn_t, epilogue=EPI_RESID, resid=dv_r)
-        dv = ops.gather_sum(dxp, slot_of, dv_r, T=T, Cc=C, k=k)
+        dgate = ops.moe_combine_bwd(dz, o, rt.slot_of, rt.top_idx, rt.top_gate, gamma, rs, d_o, dgamma, T=T, Cc=C, k=k)
+        dxp, dw1s, db1s, dw2s, db2s = _moe_experts_bwd(d_o, v, h, rt.pair_token, rt.grouped, rt.segs, w1, w2, E, ctx.packs)
+        dv_r, dwp, dbp, dsim, dtau, dwn = router_backward(rt, v, dgate, dloss, wp_t=ctx.packs.get('wp_t'))
+        dv = ops.gather_sum(dxp, rt.slot_of, dv_r, T=T, Cc=C, k=k)
         dx, ddww, ddwb, dlnw, dlnb = _block_front_bwd(dv, dout if ctx.shortcut else None, x, u, stats, dww, lnw)
-        if dwn is None and ctx.has_noise_param:
-            dwn = torch.zeros((C, E), device=dev, dtype=torch.float32)
         grads_e = [dw1s[e] for e in range(E)] + [db1s[e] for e in range(E)] + [dw2s[e] for e in range(E)] + \
                   [db2s[e] for e in range(E)]
         return (dx, ddww, ddwb, dlnw, dlnb, dgamma, dwp, dbp, dsim, dtau, dwn, None, None, None, None, None, None, None,

@@ -20,6 +20,7 @@ import torch.nn as nn
 from . import functional as Fn
 from . import lsk_functional as LF
 from .backbone import CosineTopKGate
+from .moe_routing import gating_noise
 from .registry import ROTATED_BACKBONES, BaseModule
 
 
@@ -82,13 +83,7 @@ class MoE_layer(nn.Module):
         return ws + bs
 
     def forward(self, x, gamma=None, resid=None, row_scale=None, record=None):
-        noise = None
-        if self.noisy_gating and self.training:
-            noise = getattr(self, '_injected_noise', None)
-            if noise is None:
-                T = x.numel() // x.shape[-1]
-                noise = torch.randn((T, self.num_experts), device=x.device, dtype=torch.float32)
-            noise = noise.to(x.device, torch.float32).contiguous()
+        noise = gating_noise(self, x.numel() // x.shape[-1], x.device)
         g = self.w_gate
         return LF.MoELinearFn.apply(x, g.cosine_projector.weight, g.cosine_projector.bias, g.sim_matrix, g.temperature,
                                     self.w_noise, noise, gamma, resid, row_scale, self.num_experts, self.k, record,

@@ -18,18 +18,12 @@ import torch.distributed as dist
 from torch.autograd import Function
 
 from . import ops
+from .functional import _taps, _taps_flipped
+from .moe_routing import Routing, route, router_backward
 from .ops import EPI_GELU
 
 
 AMAX_RECORD = None   # parity tests set this to a list: LSKSelectFn appends the channel argmax [T] of every LSKblock (forward order)
-
-
-def _taps(w):              # [C,1,ks,ks] -> [ks*ks][C]
-    return w.reshape(w.shape[0], -1).t().contiguous()
-
-
-def _taps_flipped(w):
-    return w.flip(2, 3).reshape(w.shape[0], -1).t().contiguous()
 
 
 def _sync_active(sync):
@@ -328,75 +322,43 @@ class MoELinearFn(Function):
         ws, bs = experts[:E], experts[E:]
         Cout = ws[0].shape[0]
         train = any(ctx.needs_input_grad)
-        r = ops.moe_router(x2, wp, bp, sim, tau, T=T, Cc=Cin, E=E, k=k, w_noise=w_noise, noise=noise, save=train)
-        plan = ops.moe_plan(r['partials'], T=T, E=E, k=k)
-        slot_of, pair_token = ops.moe_assign(r['top_idx'], plan, T=T, E=E, k=k)
-        R = plan['max_rows']
-        grouped = (plan['tile_group'], plan['num_m_tiles'])
+        rt = route(x2, wp, bp, sim, tau, w_noise, noise, E, k, save=train)
+        R = rt.rows
         w0 = ws[0].view(Cout, Cin)
         o = torch.zeros((R, Cout), device=x.device, dtype=torch.float32)
-        ops.linear_fwd(x2, w0, bs[0], out=o, row_index=pair_token, rows=R, grouped=grouped, w_group_stride=Cout * Cin,
+        ops.linear_fwd(x2, w0, bs[0], out=o, row_index=rt.pair_token, rows=R, grouped=rt.grouped, w_group_stride=Cout * Cin,
                        bias_group_stride=Cout)
         res2 = None if resid is None else resid.contiguous().view(T, Cout)
-        out, y = ops.moe_combine(o, slot_of, r['top_idx'], r['top_gate'], gamma, res2, row_scale, T=T, Cc=Cout, k=k,
+        out, y = ops.moe_combine(o, rt.slot_of, rt.top_idx, rt.top_gate, gamma, res2, row_scale, T=T, Cc=Cout, k=k,
                                  want_y=record is not None)
         if record is not None:
-            record.append(dict(x=x2, top_idx=r['top_idx'], top_gate=r['top_gate'], importance=plan['importance'],
-                               load=plan['load'], loss=plan['loss'], y=y, counts=plan['counts']))
+            record.append(dict(x=x2, y=y, **rt.record()))
         if train:
-            ctx.noisy = noise is not None     # gates depend on w_noise whenever noise was added, also for k == E
-            ctx.save_for_backward(x2, o, wp, sim, tau, gamma, row_scale, r['top_idx'], r['top_gate'], r['logits'], r['p'],
-                                  slot_of, pair_token, plan['importance'], plan['seg_begin'], plan['seg_end'],
-                                  plan['tile_group'], plan['num_m_tiles'], w0, noise, r['sigma'], r['top_vals'],
-                                  r['top_idx_m'], plan['load'], w_noise)
-            ctx.E, ctx.k, ctx.R, ctx.lead = E, k, R, tuple(lead)
+            rt.save(ctx, x2, o, gamma, row_scale, w0)
+            ctx.lead = tuple(lead)
             ctx.wshape = tuple(ws[0].shape)
-            ctx.has_noise_param = w_noise is not None
             ctx.has_resid = resid is not None
-        return out.view(*lead, Cout), plan['loss'].reshape(())
+        return out.view(*lead, Cout), rt.loss.reshape(())
 
     @staticmethod
     def backward(ctx, dout, dloss):
-        (x2, o, wp, sim, tau, gamma, rs, top_idx, top_gate, logits, p, slot_of, pair_token, importance, seg_begin, seg_end,
-         tile_group, num_m_tiles, w0, noise, sigma, top_vals, top_idx_m, load, w_noise) = ctx.saved_tensors
-        E, k, R = ctx.E, ctx.k, ctx.R
+        (x2, o, gamma, rs, w0), rt = Routing.load(ctx)
+        E, k, R = rt.E, rt.k, rt.rows
         T, Cin = x2.shape
         Cout = w0.shape[0]
         dev = x2.device
         dz = dout.contiguous().view(T, Cout)
-        grouped, segs = (tile_group, num_m_tiles), (seg_begin, seg_end)
         d_o = torch.zeros((R, Cout), device=dev, dtype=torch.float32)
         dgamma = None if gamma is None else torch.zeros((Cout,), device=dev, dtype=torch.float32)
-        dgate = ops.moe_combine_bwd(dz, o, slot_of, top_idx, top_gate, gamma, rs, d_o, dgamma, T=T, Cc=Cout, k=k)
+        dgate = ops.moe_combine_bwd(dz, o, rt.slot_of, rt.top_idx, rt.top_gate, gamma, rs, d_o, dgamma, T=T, Cc=Cout, k=k)
         dws = torch.zeros((E, Cout, Cin), device=dev, dtype=torch.float32)
-        ops.linear_wgrad(d_o, x2, dws, rows=R, x_row_index=pair_token, segs=segs, num_groups=E)
+        ops.linear_wgrad(d_o, x2, dws, rows=R, x_row_index=rt.pair_token, segs=rt.segs, num_groups=E)
         dbs = torch.zeros((E, Cout), device=dev, dtype=torch.float32)
-        ops.colsum(d_o, dbs, rows=R, Cc=Cout, segs=segs, groups=E)
+        ops.colsum(d_o, dbs, rows=R, Cc=Cout, segs=rt.segs, groups=E)
         dxp = torch.zeros((R, Cin), device=dev, dtype=torch.float32)
-        ops.linear_dgrad(d_o, w0, out=dxp, grouped=grouped, w_group_stride=Cout * Cin)
-        P = wp.shape[0]
-        dtau = torch.zeros((1,), device=dev, dtype=torch.float32)
-        dsim = torch.zeros((P, E), device=dev, dtype=torch.float32)
-        lscale = dloss.reshape(1).contiguous().float()
-        noisy = dict(noise=noise, sigma=sigma, top_vals=top_vals, top_idx_m=top_idx_m, load=load) if ctx.noisy else None
-        dp, dr = ops.moe_router_bwd(p, sim, tau, top_idx, top_gate, dgate, logits, importance, lscale, dsim, dtau, T=T,
-                                    E=E, k=k, noisy=noisy)
-        dwp = torch.zeros_like(wp)
-        ops.linear_wgrad(dp, x2, dwp)
-        dbp = torch.zeros((P,), device=dev, dtype=torch.float32)
-        ops.colsum(dp, dbp, rows=T, Cc=P)
-        dx_r = ops.linear_dgrad(dp, wp)
-        dwn = None
-        if ctx.noisy:
-            wn_t = torch.zeros((32, Cin), device=dev, dtype=torch.float32)
-            wn_t[:E] = w_noise.t()
-            dwn_t = torch.zeros((32, Cin), device=dev, dtype=torch.float32)
-            ops.linear_wgrad(dr, x2, dwn_t)
-            dwn = dwn_t[:E].t().contiguous()
-            dx_r = ops.linear_dgrad(dr, wn_t, epilogue=ops.EPI_RESID, resid=dx_r)
-        dx = ops.gather_sum(dxp, slot_of, dx_r, T=T, Cc=Cin, k=k)
-        if dwn is None and ctx.has_noise_param:
-            dwn = torch.zeros((Cin, E), device=dev, dtype=torch.float32)
+        ops.linear_dgrad(d_o, w0, out=dxp, grouped=rt.grouped, w_group_stride=Cout * Cin)
+        dx_r, dwp, dbp, dsim, dtau, dwn = router_backward(rt, x2, dgate, dloss)
+        dx = ops.gather_sum(dxp, rt.slot_of, dx_r, T=T, Cc=Cin, k=k)
         dresid = dout if ctx.has_resid else None
         grads_e = [dws[e].view(ctx.wshape) for e in range(E)] + [dbs[e] for e in range(E)]
         return (dx.view(*ctx.lead, Cin), dwp, dbp, dsim, dtau, dwn, None, dgamma, dresid, None, None, None, None, *grads_e)

@@ -1,4 +1,4 @@
-"""Expert-parallel MoE over NVLink peer memory (BASELINE config 4 mechanism) on >= 2 GPUs of one box."""
+"""Expert-parallel MoE over NVLink peer memory (BASELINE config 4 mechanism): one rank, and two GPUs of one box."""
 import os
 import subprocess
 import sys
@@ -10,9 +10,9 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 pytestmark = pytest.mark.gpu
 
 
-@pytest.mark.skipif(torch.cuda.device_count() < 2, reason='needs >= 2 GPUs')
-def test_expert_parallel_matches_local_experts():
-    n = 2
+@pytest.mark.parametrize('n', [pytest.param(n, marks=pytest.mark.skipif(torch.cuda.device_count() < n,
+                                                                         reason=f'needs >= {n} GPUs')) for n in (1, 2)])
+def test_expert_parallel_matches_local_experts(n):
     r = subprocess.run([sys.executable, '-m', 'torch.distributed.run', '--nnodes=1', '--nproc-per-node', str(n),
                         '--master-addr', '127.0.0.1', '--master-port', '29543',
                         os.path.join(ROOT, 'tests', 'dist', 'ep_gpu_worker.py'), ROOT],
