@@ -88,7 +88,8 @@ int sm3_gemm(const sm3_gemm_args* args, void* stream);
 /* Weights are constant across the tokens of a step: split them into bf16 hi/lo ONCE per optimizer step, already
  * in the tile order / swizzle the kernel's shared-memory stages use, so the GEMM brings a whole k-block of B in
  * with a single cp.async.bulk.  B(n,k) is read at B + n*stride_mn + k*stride_k (any majorness: the forward uses
- * W[N,K], the dgrad the same storage as B(n=k', k=n')).  Output: sm3_gemm_packed_elems(N,K) bf16 per group. */
+ * W[N,K], the dgrad the same storage as B(n=k', k=n')).  Output: sm3_gemm_packed_elems(N,K) bf16 per group; N is
+ * padded to whole tiles of sm3_gemm_tile_n(N) rows and the padding rows are written as zeros. */
 int64_t sm3_gemm_packed_elems(int32_t N, int32_t K);
 int sm3_gemm_pack_b(const float* B, int64_t stride_mn, int64_t stride_k, int64_t group_stride, int32_t groups,
                     int32_t N, int32_t K, uint16_t* out, void* stream);
@@ -99,7 +100,9 @@ int sm3_gemm_pack_b(const float* B, int64_t stride_mn, int64_t stride_k, int64_t
 int64_t sm3_gemm_packed_act_elems(int64_t rows, int32_t cols, int32_t mn_major, int32_t tile);
 int sm3_gemm_pack_act(const float* X, int64_t ld, const int32_t* row_index, int64_t rows, int32_t cols,
                       int32_t mn_major, int32_t tile, uint16_t* out, void* stream);
-int32_t sm3_gemm_tile_n(int32_t N);   /* tile width the GEMM uses for an N-column output (0 if unsupported) */
+/* Tile width the GEMM uses for an N-column output: the largest of 128/96/64/32 dividing N; for any other N % 8 == 0 the
+ * last tile is padded and masked (fewest tiles, then least padding); 0 if N % 8 != 0. */
+int32_t sm3_gemm_tile_n(int32_t N);
 /* Same image with an explicit tile width (N % tile == 0): the fused FFN kernels stream weight chunks of their own width. */
 int sm3_gemm_pack_b_tile(const float* B, int64_t stride_mn, int64_t stride_k, int64_t group_stride, int32_t groups,
                          int32_t N, int32_t K, int32_t tile, uint16_t* out, void* stream);

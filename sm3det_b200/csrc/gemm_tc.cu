@@ -11,28 +11,39 @@ int pick_bn(int N) {
   static const int cand[] = {128, 96, 64, 32};   // MAX_BN = 128
   for (int bn : cand)
     if (N % bn == 0) return bn;
-  return 0;
+  if (N <= 0 || N % 8) return 0;
+  // column tail: the last N-tile runs padded and masked.  Fewest tiles, then the least padding (N = 16 -> 32, 80 -> 96).
+  int best = 0, best_tiles = 0;
+  for (int bn : cand) {
+    const int tiles = (N + bn - 1) / bn;
+    if (!best || tiles < best_tiles || (tiles == best_tiles && tiles * bn < best_tiles * best)) { best = bn; best_tiles = tiles; }
+  }
+  return best;
 }
 
 static bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15u) == 0; }
 
 long long packed_elems(int N, int K) {
   const long long kblocks = (K + BK - 1) / BK;
-  return (long long)N * kblocks * BK * 2;     // hi + lo planes, K padded to a multiple of 32
+  const int bn = pick_bn(N);
+  const long long rows = bn > 0 ? (long long)(N + bn - 1) / bn * bn : N;   // N padded to whole tiles (column tail)
+  return rows * kblocks * BK * 2;             // hi + lo planes, K padded to a multiple of 32
 }
 
-// one thread per 16-byte chunk (8 k-values of one row)
+// one thread per 16-byte chunk (8 k-values of one row); rows [N, rows) of the last tile are written as zeros
 __global__ void __launch_bounds__(256) pack_b_kernel(const float* __restrict__ B, long long s_mn, long long s_k,
-                                                    long long group_stride, int N, int K, int BN, uint16_t* __restrict__ out,
+                                                    long long group_stride, int N, int rows, int K, int BN,
+                                                    uint16_t* __restrict__ out, long long out_group_stride,
                                                     long long chunks_per_group) {
   const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= chunks_per_group) return;
   const int g = blockIdx.y;
   const int kblocks = (K + BK - 1) / BK;
   // chunk index -> (row n fastest, then chunk c, then k-block): consecutive threads read consecutive rows
-  const int n = (int)(i % N);
-  const long long r = i / N;
+  const int n = (int)(i % rows);
+  const long long r = i / rows;
   const int c = (int)(r % 4), kb = (int)(r / 4);
+  const bool live = n < N;
   const float* src = B + (long long)g * group_stride + (long long)n * s_mn;
   uint32_t hi[4], lo[4];
 #pragma unroll
@@ -41,7 +52,7 @@ __global__ void __launch_bounds__(256) pack_b_kernel(const float* __restrict__ B
 #pragma unroll
     for (int q = 0; q < 2; ++q) {
       const int k = kb * BK + c * 8 + e + q;
-      v[q] = (k < K) ? __ldg(src + (long long)k * s_k) : 0.f;
+      v[q] = (live && k < K) ? __ldg(src + (long long)k * s_k) : 0.f;
     }
     const uint32_t u0 = __float_as_uint(v[0]), u1 = __float_as_uint(v[1]);
     hi[e / 2] = __byte_perm(u0, u1, 0x7632);
@@ -50,7 +61,7 @@ __global__ void __launch_bounds__(256) pack_b_kernel(const float* __restrict__ B
     lo[e / 2] = __byte_perm(r0, r1, 0x7632);
   }
   const int nt = n / BN, row = n % BN;
-  uint8_t* tile = reinterpret_cast<uint8_t*>(out + (long long)g * ((long long)N * kblocks * BK * 2)) +
+  uint8_t* tile = reinterpret_cast<uint8_t*>(out + (long long)g * out_group_stride) +
                   ((long long)nt * kblocks + kb) * ((long long)BN * 128);
   const uint32_t o = kmajor_sw64_offset((uint32_t)row, (uint32_t)c);
   *reinterpret_cast<uint4*>(tile + o) = make_uint4(hi[0], hi[1], hi[2], hi[3]);
@@ -61,12 +72,15 @@ int pack_b(const float* B, long long s_mn, long long s_k, long long group_stride
            uint16_t* out, cudaStream_t stream, int tile) {
   SM3_REQUIRE(B && out && N > 0 && K > 0 && groups >= 1, SM3_ERR_INVALID_ARG, "gemm pack: bad argument");
   const int BN = tile > 0 ? tile : pick_bn(N);
-  SM3_REQUIRE(BN > 0 && BN % 8 == 0 && BN <= 256 && N % BN == 0, SM3_ERR_UNSUPPORTED_SHAPE, "gemm pack: N=%d has no tile width (tile=%d)", N, tile);
+  // an explicit tile must divide N; the default tile may leave a column tail, whose image rows are padded with zeros
+  SM3_REQUIRE(BN > 0 && BN % 8 == 0 && BN <= 256 && (tile > 0 ? N % BN == 0 : N % 8 == 0), SM3_ERR_UNSUPPORTED_SHAPE,
+              "gemm pack: N=%d has no tile width (tile=%d)", N, tile);
   SM3_REQUIRE((reinterpret_cast<uintptr_t>(out) & 15u) == 0, SM3_ERR_INVALID_ARG, "gemm pack: output must be 16B aligned");
   const long long kblocks = (K + BK - 1) / BK;
-  const long long chunks = (long long)N * kblocks * 4;
+  const int rows = (N + BN - 1) / BN * BN;
+  const long long chunks = (long long)rows * kblocks * 4;
   dim3 grid((unsigned)((chunks + 255) / 256), (unsigned)groups);
-  pack_b_kernel<<<grid, 256, 0, stream>>>(B, s_mn, s_k, group_stride, N, K, BN, out, chunks);
+  pack_b_kernel<<<grid, 256, 0, stream>>>(B, s_mn, s_k, group_stride, N, rows, K, BN, out, packed_elems(N, K), chunks);
   return check_launch("pack_b_kernel");
 }
 
@@ -189,8 +203,8 @@ int launch(Params p, cudaStream_t stream) {
   SM3_REQUIRE((p.b_smn == 1) != (p.b_sk == 1), SM3_ERR_INVALID_ARG, "gemm: B needs exactly one unit stride");
   const bool a_mn = (p.a_smn == 1 && p.a_sk != 1), b_mn = (p.b_smn == 1 && p.b_sk != 1);
   if (p.BN == 0) p.BN = pick_bn(p.N);
-  SM3_REQUIRE(p.BN >= 32 && p.BN <= MAX_BN && p.BN % 32 == 0 && p.N % p.BN == 0, SM3_ERR_UNSUPPORTED_SHAPE,
-              "gemm: N=%d has no tile width (multiple of 32 <= 128 dividing N)", p.N);
+  SM3_REQUIRE(p.BN >= 32 && p.BN <= MAX_BN && p.BN % 32 == 0 && p.N % 8 == 0, SM3_ERR_UNSUPPORTED_SHAPE,
+              "gemm: N=%d has no tile width (N a multiple of 8, tile width a multiple of 32 <= 128)", p.N);
   SM3_REQUIRE(aligned16(p.A) && aligned16(p.B) && aligned16(p.D), SM3_ERR_INVALID_ARG, "gemm: pointers must be 16B aligned");
   if (!a_mn) SM3_REQUIRE(p.a_smn % 4 == 0 && p.K % 4 == 0, SM3_ERR_UNSUPPORTED_SHAPE, "gemm: K-major A needs K%%4==0, lda%%4==0");
   else       SM3_REQUIRE(p.a_sk % 4 == 0 && p.M % 8 == 0, SM3_ERR_UNSUPPORTED_SHAPE, "gemm: MN-major A needs M%%8==0, lda%%4==0");
@@ -207,7 +221,7 @@ int launch(Params p, cudaStream_t stream) {
   if (p.epi & EPI_COLSUM) SM3_REQUIRE(p.colsum && aligned16(p.colsum) && p.colsum_group_stride % 4 == 0, SM3_ERR_INVALID_ARG, "gemm: colsum");
   if (p.epi & EPI_RESID) SM3_REQUIRE(p.resid && aligned16(p.resid) && p.ld_resid % 4 == 0, SM3_ERR_INVALID_ARG, "gemm: resid");
 
-  p.n_tiles = p.N / p.BN;
+  p.n_tiles = (p.N + p.BN - 1) / p.BN;      // a column tail runs as one more, padded and masked, tile
   p.m_tiles = (p.M + BM - 1) / BM;
   if (p.sched == SCHED_DENSE) {
     p.k_splits = 1; p.num_groups = 1;

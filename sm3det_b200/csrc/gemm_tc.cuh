@@ -68,6 +68,9 @@ struct Params {
   // pre-split weights (see pack_b): tile-ordered bf16 hi/lo images brought in with one cp.async.bulk per k-block
   const uint16_t* b_packed; long long b_packed_group_stride;   // stride in bf16 elements
   const uint16_t* a_packed;   // pre-split activation image (pack_a); with b_packed the whole main loop is bulk copies
+  // Column tail: N need only be a multiple of 8.  When BN does not divide N the last N-tile is padded to BN columns: its
+  // B rows past N load as zeros (the fp32 producers skip them, pack_b writes zero rows, pack_act zero columns) and the
+  // epilogue masks every per-column access at n >= N (bias, col_scale, aux, resid, D, colsum).
   int M, N, K, BN;
   // schedule
   int sched;
@@ -297,7 +300,7 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) gemm_bf16x3_kernel(const __gri
 #pragma unroll
         for (int it = 0; it < 2; ++it) {
           const int row = row0 + it * 8 + rl;
-          dst[it] = (row < p.M) ? ldg_f4(p.resid + (long long)row * p.ld_resid + n_) : make_float4(0.f, 0.f, 0.f, 0.f);
+          dst[it] = (row < p.M && n_ < p.N) ? ldg_f4(p.resid + (long long)row * p.ld_resid + n_) : make_float4(0.f, 0.f, 0.f, 0.f);
         }
       };
       if (EPI & EPI_RESID) load_resid(0, rr);
@@ -373,15 +376,16 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) gemm_bf16x3_kernel(const __gri
         if ((EPI & EPI_RESID) && c + 1 < nchunks) load_resid(c + 1, rn);
         __syncwarp();
         const int n = tl.n0 + c * EPI_CW + c4;
+        const bool n_ok = n < p.N;           // column tail: N % 8 == 0, so a lane's 4 columns are all in or all out
         float4 bv = make_float4(0.f, 0.f, 0.f, 0.f), sv = make_float4(1.f, 1.f, 1.f, 1.f);
-        if (EPI & EPI_BIAS) bv = ldg_f4(bias + n);
-        if (EPI & EPI_COLSCALE) sv = ldg_f4(p.col_scale + n);
+        if ((EPI & EPI_BIAS) && n_ok) bv = ldg_f4(bias + n);
+        if ((EPI & EPI_COLSCALE) && n_ok) sv = ldg_f4(p.col_scale + n);
         float4 cs = make_float4(0.f, 0.f, 0.f, 0.f);
 #pragma unroll
         for (int it = 0; it < 2; ++it) {
           const int r = it * 8 + rl;
           const int row = row0 + r;
-          if (row >= p.M) continue;
+          if (row >= p.M || !n_ok) continue;
           float4 x;
           asm volatile("ld.shared.v4.f32 {%0, %1, %2, %3}, [%4];"
                        : "=f"(x.x), "=f"(x.y), "=f"(x.z), "=f"(x.w)
@@ -416,7 +420,7 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) gemm_bf16x3_kernel(const __gri
             cs.x += __shfl_xor_sync(0xffffffffu, cs.x, o); cs.y += __shfl_xor_sync(0xffffffffu, cs.y, o);
             cs.z += __shfl_xor_sync(0xffffffffu, cs.z, o); cs.w += __shfl_xor_sync(0xffffffffu, cs.w, o);
           }
-          if (lane < 4) {
+          if (lane < 4 && n_ok) {
             if (cs_smem) {
               const uint32_t sa = cs_base + 4u * (uint32_t)n;
               asm volatile("red.shared.add.f32 [%0], %1;" ::"r"(sa), "f"(cs.x) : "memory");
@@ -665,7 +669,8 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) gemm_bf16x3_kernel(const __gri
 
 // Pre-split a weight operand B(n,k) (element at ptr + n*s_mn + k*s_k, `groups` matrices `group_stride` apart) into
 // the tile-ordered bf16 image the kernel bulk-copies: [group][n_tile][k_block]{ hi[BN x 32] | lo[BN x 32] } with
-// each plane in the K-major SWIZZLE_64B canonical layout.  packed_elems(N, K) bf16 elements per group.
+// each plane in the K-major SWIZZLE_64B canonical layout.  packed_elems(N, K) bf16 elements per group: N is padded to
+// whole tiles of pick_bn(N) rows, and the padding rows are written as zeros.
 long long packed_elems(int N, int K);
 // `tile` > 0 overrides the tile width (the fused FFN kernels stream weight chunks of their own width).
 int pack_b(const float* B, long long s_mn, long long s_k, long long group_stride, int groups, int N, int K,
@@ -678,7 +683,8 @@ int pack_act(const float* X, long long ld, const int* row_index, long long rows,
              uint16_t* out, cudaStream_t stream);
 // Host-side launcher (gemm_tc.cu): validates shapes, fills derived fields, launches on `stream`.
 int launch(Params p, cudaStream_t stream);
-// Picks the largest supported tile width that divides N (multiple of 32, <= 256); 0 if none.
+// Tile width of an N-column output: the largest of {128, 96, 64, 32} that divides N; for other N % 8 == 0 (column
+// tail) the one with the fewest tiles, then the least padding; 0 if N % 8 != 0.
 int pick_bn(int N);
 
 }  // namespace gemm

@@ -163,8 +163,8 @@ class Mlp(nn.Module):
 class LSKblock(nn.Module):
     def __init__(self, dim):
         super().__init__()
-        if dim % 64:
-            raise NotImplementedError(f'sm3det_b200: LSKNet width {dim} unsupported (multiple of 64)')
+        if dim % 32:     # the depthwise convs need C % 32; the dim/2-wide 1x1 convs run on the GEMM's column tail
+            raise NotImplementedError(f'sm3det_b200: LSKNet width {dim} unsupported (multiple of 32)')
         self.conv0 = nn.Conv2d(dim, dim, 5, padding=2, groups=dim)
         self.conv_spatial = nn.Conv2d(dim, dim, 7, stride=1, padding=9, groups=dim, dilation=3)
         self.conv1 = nn.Conv2d(dim, dim // 2, 1)

@@ -89,10 +89,18 @@ def _pi(t):
 
 
 def _pick_bn(n: int) -> int:
+    """Tile width of an n-column GEMM output, as gemm::pick_bn: the largest of 128/96/64/32 dividing n; for any other
+    n % 8 == 0 the last tile runs padded and masked, with the fewest tiles and then the least padding."""
     for bn in (128, 96, 64, 32):
         if n % bn == 0:
             return bn
-    raise ValueError(f'N={n} has no GEMM tile width (multiple of 32)')
+    if n > 0 and n % 8 == 0:
+        return min((128, 96, 64, 32), key=lambda bn: (-(-n // bn), -(-n // bn) * bn))
+    raise ValueError(f'N={n} has no GEMM tile width (multiple of 8)')
+
+
+def _n_tiles(n: int) -> int:
+    return -(-n // _pick_bn(n))
 
 
 def num_sms() -> int:
@@ -129,7 +137,8 @@ def gemm(*, A, a_smn, a_sk, B, b_smn, b_sk, M, N, K, D, ldd, b_group_stride=0, a
 
 def pack_weight(w, *, transposed: bool, groups: int = 1, out=None, tile: int = 0):
     """bf16 hi/lo tile image of a weight for the GEMM's B operand (sm3_gemm_pack_b) -> (buffer, elems_per_group).
-    tile > 0: explicit tile width (the fused FFN kernels stream weight chunks of their own width).
+    tile > 0: explicit tile width (the fused FFN kernels stream weight chunks of their own width).  The image holds N
+    padded to whole tiles of _pick_bn(N) rows (zeros past N), so a column tail (N % 32 != 0) takes the packed path too.
 
     w: [N,K] (or the first of `groups` adjacent [N,K] expert weights).  transposed=False packs B(n,k) = w[n,k]
     (forward);  transposed=True packs B(n=k', k=n') = w[n',k'] (dgrad).  Callers cache the result per parameter
@@ -262,7 +271,7 @@ PACK_W_MIN_TILES = int(_os.environ.get('SM3_PACK_W_MIN_TILES', '2'))
 
 
 def _pack_a_pays(N, K):
-    return K >= PACK_A_MIN_K and (N // _pick_bn(N)) >= 2 or K >= 4 * PACK_A_MIN_K
+    return K >= PACK_A_MIN_K and _n_tiles(N) >= 2 or K >= 4 * PACK_A_MIN_K
 
 
 def linear_fwd(x, w, bias=None, *, epilogue=0, out=None, aux_out=None, col_scale=None, row_scale=None, resid=None,
@@ -329,13 +338,13 @@ def linear_wgrad(dy, x, dw, *, rows=None, x_row_index=None, row_scale=None, segs
     R = rows if rows is not None else dy.shape[0]
     N = dw.shape[-2]
     K = dw.shape[-1]
-    tiles = ((N + 127) // 128) * (K // _pick_bn(K)) * num_groups
+    tiles = ((N + 127) // 128) * _n_tiles(K) * num_groups
     # ~3 work items per SM (the per-expert segments are unequal), but at least 1024 reduction rows per split
     splits = -(-3 * num_sms() // max(1, tiles))
     splits = max(1, min(64 if tiles > 1 else 2 * num_sms(), splits, max(1, (R // num_groups) // 1024)))
     epi = EPI_ATOMIC | (EPI_ROWSCALE if row_scale is not None else 0)
     kw = {}
-    if dy_packed is not None or x_packed is not None or ((N + 127) // 128) * (K // _pick_bn(K)) >= PACK_W_MIN_TILES:
+    if dy_packed is not None or x_packed is not None or ((N + 127) // 128) * _n_tiles(K) >= PACK_W_MIN_TILES:
         # both operands are re-read by several output tiles: split them once (MN-major images), gather included
         if dy_packed is None:
             dy_packed = pack_act(dy, rows=R, cols=N, mn_major=True, tile=128)
