@@ -120,6 +120,10 @@ size_t sm3_gemm_workspace_bytes(const sm3_gemm_args* args);
  *                        A1 = v, Wa1 = W1 [4C,C], Wb = W2 [C,4C]
  *   mode 1 (backward dv) out = ((A2 Wa2^T) * gelu'(A1 Wa1^T + b1)) Wb^T      (the hidden pre-activation is recomputed)
  *                        A1 = v, A2 = dz, Wa1 = W1, Wa2 = (gamma W2)^T stored [4C,C], Wb = W1^T stored [C,4C]
+ *   mode 2 (backward dv + weight-gradient operands, C <= 128) mode 1, and also dh_mn / act_mn = the MN-major images
+ *                        (sm3_gemm_packed_act_elems(M, 4C, 1, 128) elements each) of dh = (A2 Wa2^T) * gelu'(h) and of
+ *                        gelu(h), rows M .. ceil32(M) zero; db1 += column sums of dh
+ *   mode 3 (as mode 2, C = 192)  h is read from h_in (the forward's h_out) instead of recomputed; a1 / wa1 are unused
  * a1 / a2: K-major images from sm3_gemm_pack_act(tile 128) or sm3_layernorm_fwd_img; wa1 / wa2: sm3_gemm_pack_b_tile(tile =
  * chunk) of the [4C,C] matrices; wb: sm3_gemm_pack_b_tile(tile = C) of the [C,4C] matrix; chunk = sm3_ffn_fused_chunk(mode, C). */
 typedef struct sm3_ffn_args {
@@ -134,6 +138,9 @@ typedef struct sm3_ffn_args {
   float* aux_out;                  /* [M,C] mode 0, optional */
   float* h_out;                    /* [M,4C] mode 0, optional: hidden pre-activation, for the GEMM-based backward */
   int32_t M, C, H4, chunk, mma_passes, mode;
+  uint16_t* dh_mn; uint16_t* act_mn;   /* modes 2, 3 */
+  float* db1;                      /* [4C] modes 2, 3: accumulated into */
+  const float* h_in;               /* [M,4C] mode 3 */
 } sm3_ffn_args;
 int32_t sm3_ffn_fused_chunk(int32_t mode, int32_t C);   /* hidden chunk width for (mode, C); 0 = shape not supported */
 int sm3_ffn_fused(const sm3_ffn_args* args, void* stream);

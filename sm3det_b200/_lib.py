@@ -64,6 +64,7 @@ class FfnArgs(C.Structure):
         ('out', c_f32p), ('aux_out', c_f32p), ('h_out', c_f32p),
         ('M', C.c_int32), ('C', C.c_int32), ('H4', C.c_int32), ('chunk', C.c_int32), ('mma_passes', C.c_int32),
         ('mode', C.c_int32),
+        ('dh_mn', C.c_void_p), ('act_mn', C.c_void_p), ('db1', c_f32p), ('h_in', c_f32p),
     ]
 
 

@@ -118,7 +118,9 @@ class PackCache:
     def invalidate(self):
         self._d.clear()
 
-    def get(self, name, params, transposed, tile=0):
+    def get(self, name, params, transposed, tile=0, src=None):
+        """Image of params[0] (as `groups = len(params)` adjacent weights), or of the one matrix `src()` derives from params
+        (e.g. gamma * W2), rebuilt whenever any of params changed."""
         from . import ops
         key = tuple(p._version for p in params) + (params[0].data_ptr(), str(params[0].device))
         name = (name, tile)
@@ -127,7 +129,8 @@ class PackCache:
             return hit[1]
         reuse = None if hit is None or hit[1][0].device != params[0].device else hit[1][0]   # never write into a buffer
         with torch.no_grad():                                                                # left behind on another GPU
-            packed = ops.pack_weight(params[0], transposed=transposed, groups=len(params), out=reuse, tile=tile)
+            w, groups = (params[0], len(params)) if src is None else (src(), 1)
+            packed = ops.pack_weight(w, transposed=transposed, groups=groups, out=reuse, tile=tile)
         self._d[(name, transposed)] = (key, packed)
         return packed
 
@@ -199,7 +202,20 @@ class ConvNeXtBlock(nn.Module):
             else:
                 packs = {'w1': pc.get('w1', [w1], False), 'w2': pc.get('w2', [w2], False)}
             if grad:
-                packs['w1_t'] = pc.get('w1', [w1], True)
+                # backward: the chain kernel forms dv, both weight-gradient operands and db1 in one pass (mode 2 recomputes
+                # h from v, mode 3 reads the h the forward saved); otherwise dgrad -> act_pack -> dgrad
+                cb, bmode = (ops.ffn_chunk(2, C), 2) if cf > 0 else (0, 0)
+                if cf > 0 and cb == 0:
+                    cb, bmode = ops.ffn_chunk(3, C), 3
+                if cb > 0:
+                    packs['fused'].update(bwd=cb, bwd_mode=bmode)
+                    if bmode == 2:
+                        packs['w1_cb'] = pc.get('w1', [w1], False, tile=cb)
+                    g = self.gamma
+                    packs['w2g_t'] = pc.get('w2g', [w2, g], True, tile=cb, src=lambda: ops.scale_rows(w2, row_scale=g))
+                    packs['w1_tn'] = pc.get('w1', [w1], True, tile=C)
+                else:
+                    packs['w1_t'] = pc.get('w1', [w1], True)
             packs['grad'] = grad
             packs['shortcut'] = shortcut
             packs['checkpoint'] = checkpoint

@@ -64,7 +64,7 @@ int sm3_gemm_pack_b_tile(const float* B, int64_t s_mn, int64_t s_k, int64_t grou
 }
 size_t sm3_gemm_workspace_bytes(const sm3_gemm_args*) { return 0; }
 
-int32_t sm3_ffn_fused_chunk(int32_t mode, int32_t C) { return (mode == 0 || mode == 1) ? ffn::chain_chunk(mode, C) : 0; }
+int32_t sm3_ffn_fused_chunk(int32_t mode, int32_t C) { return (mode >= 0 && mode <= 3) ? ffn::chain_chunk(mode, C) : 0; }
 size_t sm3_ffn_fused_workspace_bytes(const sm3_ffn_args*) { return 0; }
 int sm3_ffn_fused(const sm3_ffn_args* a, void* stream) {
   if (!a) { set_last_error("sm3_ffn_fused: null args"); return SM3_ERR_INVALID_ARG; }
@@ -72,6 +72,7 @@ int sm3_ffn_fused(const sm3_ffn_args* a, void* stream) {
   p.a1 = a->a1; p.a2 = a->a2; p.wa1 = a->wa1; p.wa2 = a->wa2; p.wb = a->wb;
   p.bias1 = a->bias1; p.bias2 = a->bias2; p.col_scale = a->col_scale; p.row_scale = a->row_scale; p.resid = a->resid;
   p.out = a->out; p.aux_out = a->aux_out; p.h_out = a->h_out;
+  p.dh_mn = a->dh_mn; p.act_mn = a->act_mn; p.db1 = a->db1; p.h_in = a->h_in;
   p.M = a->M; p.C = a->C; p.H4 = a->H4; p.HC = a->chunk; p.passes = a->mma_passes; p.mode = a->mode;
   return ffn::chain(p, S(stream));
 }

@@ -16,6 +16,11 @@
 //      MODE 0 = forward (A1 = v, Wa1 = W1, Wb = W2);  MODE 1 = backward into dv (A1 = v: the hidden pre-activation is
 //      RECOMPUTED, A2 = dz, Wa1 = W1, Wa2 = (gamma W2)^T, Wb = W1^T) -- the tensor pipe has >2x slack on these shapes,
 //      HBM does not, so nothing hidden-sized is saved by the forward at all.
+//      MODE 2 = MODE 1 that also writes, from the middle stage's registers, the two weight-gradient operands as MN-major
+//      SWIZZLE_128B images (dh = d * gelu'(h) and gelu(h), 128-column tiles, rows M .. ceil32(M) zero: the layout act_pack
+//      writes) and db1 = sum_t dh (per-CTA shared-memory partials, one global atomic per column per CTA).
+//      MODE 3 = MODE 2 for C = 192, where v and dz tiles do not both fit: A2 = dz alone, h is read from the forward's
+//      saved fp32 h_in straight into the fragment layout instead of being recomputed.
 //
 // Not fused: the weight gradients (split-K GEMMs).
 #pragma once
@@ -40,6 +45,10 @@ struct ChainParams {
   float* out;             // [M, C]
   float* aux_out;         // [M, C] or null: acc_o + bias2 before scaling (y2, needed for dgamma)
   float* h_out;           // MODE 0: [M, H4] or null: hidden pre-activation A1 Wa1^T + b1 (saved for a GEMM-based backward)
+  uint16_t* dh_mn;        // MODES 2, 3: MN-major image (128-column tiles) of dh = d * gelu'(h), wgrad1's dy operand
+  uint16_t* act_mn;       // MODES 2, 3: MN-major image (128-column tiles) of gelu(h), wgrad2's x operand
+  float* db1;             // MODES 2, 3: [H4] += column sums of dh
+  const float* h_in;      // MODE 3: [M, H4] the saved pre-activation (b1 included) instead of its recompute
   int M, C, H4, HC, passes, mode;
   int debug;              // perf experiments only: bit0 = middle stage skips the GELU math, bit1 = skip the operand split/stores
 };

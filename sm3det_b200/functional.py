@@ -159,14 +159,16 @@ def _block_front_bwd(dv, dout, x, u, stats, dww, lnw):
 
 def _dense_ffn(x, v, v_img, b1, w1, w2, b2, gamma, row_scale, resid, packs, keep):
     """FFN + layer scale (+ drop-path row scale, + shortcut) of the dense block -> (out [T,C], h, y2).  keep: also return
-    what the backward reads, the pre-activation h [T,4C] and the pre-gamma output y2 [T,C] (else both None)."""
+    what the backward reads, the pre-gamma output y2 [T,C] and the pre-activation h [T,4C] (else both None; h is None too
+    when the backward recomputes it, fused bwd_mode 2)."""
     N, H, W, C = x.shape
     T = N * H * W
     fused = packs.get('fused')
     if fused is not None:
+        want_h = keep and fused.get('bwd_mode') != 2
         res = ops.ffn_fused_fwd(v_img, packs['w1_c'][0], packs['w2_n'][0], b1, b2, T=T, C=C, chunk=fused['fwd'],
-                                gamma=gamma, row_scale=row_scale, resid=resid, want_aux=keep, want_h=keep)
-        return res[0], (res[2] if keep else None), res[1]
+                                gamma=gamma, row_scale=row_scale, resid=resid, want_aux=keep, want_h=want_h)
+        return res[0], (res[2] if want_h else None), res[1]
     # GEMM1 stores the pre-activation only; GELU runs in the HBM-bound act_pack kernel, which emits the result
     # directly as GEMM2's pre-split A operand (fp32 `a` never exists)
     h = ops.linear_fwd(v, w1, b1, packed=packs.get('w1'))
@@ -182,9 +184,11 @@ def _dense_ffn(x, v, v_img, b1, w1, w2, b2, gamma, row_scale, resid, packs, keep
 @ops.captures_precision
 class DenseBlockFn(Function):
     """Dense ConvNeXt block.  Narrow stages (ops.ffn_chunk > 0: C a multiple of 32 up to 224) run the FFN forward as the fused wgmma kernel of
-    csrc/ffn_fused.cu (GEMM1 -> GELU -> GEMM2 on chip; the hidden tensor is written once, as fp32 h, only when a backward
-    follows).  The backward is the GEMM sequence (dgrad2 -> act_pack -> wgrads / dgrad1).  Wider stages keep
-    GEMM -> act_pack -> GEMM."""
+    csrc/ffn_fused.cu (GEMM1 -> GELU -> GEMM2 on chip).  Where the chain kernel has a backward mode that emits the
+    weight-gradient operands (packs['fused']['bwd_mode']: 2 at C <= 128, recomputing h from v; 3 at C = 192, reading the h
+    the forward saved), one launch forms dv, the MN-major images of dh and gelu(h) and db1, and the two split-K wgrads
+    consume the images.  Otherwise the forward saves fp32 h and the backward is the GEMM sequence
+    (dgrad2 -> act_pack -> wgrads / dgrad1).  Wider stages keep GEMM -> act_pack -> GEMM."""
 
     @staticmethod
     def forward(ctx, x, dww, dwb, lnw, lnb, w1, b1, w2, b2, gamma, row_scale, eps, packs):
@@ -217,28 +221,30 @@ class DenseBlockFn(Function):
             v_img = None
         out, h, y2 = _dense_ffn(x, v, v_img, b1, w1, w2, b2, gamma, row_scale, resid, packs, keep=train)
         if train:
-            ctx.save_for_backward(x, u, stats, v, h, y2, dww, lnw, w1, w2, gamma, row_scale)
+            if (fused or {}).get('bwd_mode') != 2:
+                v_img = None                             # only the recomputing backward reads it
+            ctx.save_for_backward(x, u, stats, v, v_img, h, y2, dww, lnw, w1, b1, w2, gamma, row_scale)
             ctx.packs = packs
         return out.view(N, H, W, C)
 
     @staticmethod
     def _recompute(ctx, x, dww, dwb, lnw, lnb, w1, b1, w2, b2, gamma, rs):
-        """Checkpointed backward: rebuild (u, stats, v, h, y2) with the forward's own kernels and arguments."""
+        """Checkpointed backward: rebuild (u, stats, v, v_img, h, y2) with the forward's own kernels and arguments."""
         N, H, W, C = x.shape
         want_img = ctx.packs.get('fused') is not None        # the plain forward's v and stats then come from layernorm_fwd_img
         u, stats, v, v_img = ops.dwconv7_ln(x, _taps(dww), dwb, lnw, lnb, ctx.eps, want_u=True, want_stats=True, want_v=True,
                                             want_img=want_img)
         resid = x.view(N * H * W, C) if ctx.shortcut else None
         _, h, y2 = _dense_ffn(x, v, v_img, b1, w1, w2, b2, gamma, rs, resid, ctx.packs, keep=True)
-        return u, stats, v, h, y2
+        return u, stats, v, v_img, h, y2
 
     @staticmethod
     def backward(ctx, dout):
         if ctx.checkpoint:
             x, dww, dwb, lnw, lnb, w1, b1, w2, b2, gamma, rs = ctx.saved_tensors
-            u, stats, v, h, y2 = DenseBlockFn._recompute(ctx, x, dww, dwb, lnw, lnb, w1, b1, w2, b2, gamma, rs)
+            u, stats, v, v_img, h, y2 = DenseBlockFn._recompute(ctx, x, dww, dwb, lnw, lnb, w1, b1, w2, b2, gamma, rs)
         else:
-            x, u, stats, v, h, y2, dww, lnw, w1, w2, gamma, rs = ctx.saved_tensors
+            x, u, stats, v, v_img, h, y2, dww, lnw, w1, b1, w2, gamma, rs = ctx.saved_tensors
         N, H, W, C = x.shape
         T = N * H * W
         dout = dout.contiguous()
@@ -252,22 +258,33 @@ class DenseBlockFn(Function):
             csum = torch.zeros((C,), device=dev, dtype=torch.float32)
             ops.colsum(dz, csum, rows=T, Cc=C, row_scale=rs)
         db2 = csum * gamma
-        w2g = ops.scale_rows(w2, row_scale=gamma)                   # gamma[c] * W2[c, :]
-        da = ops.linear_dgrad(dz, w2g, epilogue=(EPI_ROWSCALE if rs is not None else 0), row_scale=rs,
-                              packed=ops.pack_weight(w2g, transposed=True))
-        # dh = da * gelu'(h) goes straight into the two operand images (dgrad1's A, wgrad1's A) + db1 column sums
         db1 = torch.zeros((4 * C,), device=dev, dtype=torch.float32)
-        # one pass over h: dh = da * gelu'(h) as dgrad1's / wgrad1's operands (+ db1) and a = gelu(h) as wgrad2's operand
-        dh_k, dh_mn, a_mn = ops.act_pack(h, rows=T, width=4 * C, mode=ops.ACT_BWD, da=da, want_k=True, mn_tile=128,
-                                      mn_tile2=ops._pick_bn(4 * C), colsum=db1)
-        del da
         dzs = dz if rs is None else ops.scale_rows(dz, row_scale=rs)
+        fused = ctx.packs.get('fused') or {}
+        if fused.get('bwd_mode'):
+            # one chain-kernel pass: d = dzs (gamma W2) and dh = d * gelu'(h) stay on chip; out come dv, db1 and the two
+            # wgrad operand images (dh for wgrad1, gelu(h) for wgrad2)
+            dz_img = ops.pack_act(dzs, rows=T, cols=C, mn_major=False)
+            w1_cb = ctx.packs.get('w1_cb')
+            dv, dh_mn, a_mn = ops.ffn_fused_bwd(v_img, dz_img, None if w1_cb is None else w1_cb[0], ctx.packs['w2g_t'][0],
+                                                ctx.packs['w1_tn'][0], b1, T=T, C=C, chunk=fused['bwd'],
+                                                want_wgrad_images=True, db1=db1, h=h if fused['bwd_mode'] == 3 else None)
+            del dz_img, h
+        else:
+            w2g = ops.scale_rows(w2, row_scale=gamma)                   # gamma[c] * W2[c, :]
+            da = ops.linear_dgrad(dz, w2g, epilogue=(EPI_ROWSCALE if rs is not None else 0), row_scale=rs,
+                                  packed=ops.pack_weight(w2g, transposed=True))
+            # one pass over h: dh = da * gelu'(h) as dgrad1's / wgrad1's operands (+ db1) and a = gelu(h) as wgrad2's operand
+            dh_k, dh_mn, a_mn = ops.act_pack(h, rows=T, width=4 * C, mode=ops.ACT_BWD, da=da, want_k=True, mn_tile=128,
+                                          mn_tile2=ops._pick_bn(4 * C), colsum=db1)
+            del da
         dw2 = torch.zeros_like(w2)
         ops.linear_wgrad(dzs, None, dw2, rows=T, row_scale=gamma, x_packed=a_mn)
         del a_mn
         dw1 = torch.zeros_like(w1)
         ops.linear_wgrad(None, v, dw1, rows=T, dy_packed=dh_mn)
-        dv = ops.linear_dgrad(None, w1, rows=T, a_packed=dh_k, packed=ctx.packs.get('w1_t'))
+        if not fused.get('bwd_mode'):
+            dv = ops.linear_dgrad(None, w1, rows=T, a_packed=dh_k, packed=ctx.packs.get('w1_t'))
         dx, ddww, ddwb, dlnw, dlnb = _block_front_bwd(dv, dout if ctx.shortcut else None, x, u, stats, dww, lnw)
         return dx, ddww, ddwb, dlnw, dlnb, dw1, db1, dw2, db2, dgamma, None, None, None
 

@@ -176,13 +176,17 @@ ACT_GELU, ACT_DGELU, ACT_COPY, ACT_BWD = 0, 1, 2, 3
 
 
 # ---- fused dense FFN (narrow stages): the [T,4C] hidden tensor never leaves the SM --------------------------------------
-FFN_FWD, FFN_BWD_DX = 0, 1
+FFN_FWD, FFN_BWD_DX, FFN_BWD_IMG, FFN_BWD_IMG_H = 0, 1, 2, 3
 
 
 def ffn_chunk(mode: int, C: int) -> int:
-    """hidden chunk width of sm3_ffn_fused for (mode, C); 0 = not supported (use the GEMM -> act_pack -> GEMM path)."""
+    """hidden chunk width of sm3_ffn_fused for (mode, C); 0 = not supported (use the GEMM -> act_pack -> GEMM path).
+    SM3_FUSED_FFN=0 disables every mode; SM3_FUSED_FFN_BWD=0 only the backward modes that emit the weight-gradient
+    operands (2, 3), so the dense blocks' backward takes dgrad -> act_pack -> dgrad again (A/B in one process)."""
     import os
     if os.environ.get('SM3_FUSED_FFN', '1') == '0':
+        return 0
+    if mode >= FFN_BWD_IMG and os.environ.get('SM3_FUSED_FFN_BWD', '1') == '0':
         return 0
     return int(_lib.load().sm3_ffn_fused_chunk(mode, C))
 
@@ -212,14 +216,31 @@ def ffn_fused_fwd(v_img, w1_img, w2_img, b1, b2, *, T, C, chunk, gamma=None, row
     return (out, aux, h) if want_h else (out, aux)
 
 
-def ffn_fused_bwd(v_img, dz_img, w1_img, w2gt_img, w1t_img, b1, *, T, C, chunk):
-    """dv[T,C] = ((dz (gamma W2)) * gelu'(v W1^T + b1)) W1   (hidden pre-activation recomputed from v)."""
+def ffn_fused_bwd(v_img, dz_img, w1_img, w2gt_img, w1t_img, b1, *, T, C, chunk, want_wgrad_images=False, db1=None, h=None):
+    """dv[T,C] = ((dz (gamma W2)) * gelu'(v W1^T + b1)) W1   (hidden pre-activation recomputed from v).
+
+    want_wgrad_images: also return the two weight-gradient operands, (dv, dh_mn, a_mn): the MN-major images (tile 128) of
+    dh = (dz (gamma W2)) * gelu'(h) and of gelu(h) that linear_wgrad takes as dy_packed / x_packed, and add the column
+    sums of dh into db1 [4C] (required).  h: the forward's saved pre-activation [T,4C]; given, the kernel reads it instead of
+    recomputing it (mode 3; v_img and w1_img are then unused).  chunk = ffn_chunk(2 or 3, C) accordingly."""
     lib = _lib.load()
     out = torch.empty((T, C), device=b1.device, dtype=torch.float32)
-    a = _ffn_args(T=T, C=C, chunk=chunk, mode=FFN_BWD_DX, a1=v_img, a2=dz_img, wa1=w1_img, wa2=w2gt_img, b1=b1, wb=w1t_img)
-    a.out = _p(out)
+    if not want_wgrad_images:
+        a = _ffn_args(T=T, C=C, chunk=chunk, mode=FFN_BWD_DX, a1=v_img, a2=dz_img, wa1=w1_img, wa2=w2gt_img, b1=b1, wb=w1t_img)
+        a.out = _p(out)
+        _lib.check(lib.sm3_ffn_fused(_ct.byref(a), _stream()), 'sm3_ffn_fused(bwd)')
+        return out
+    if db1 is None:
+        raise ValueError('ffn_fused_bwd: want_wgrad_images needs db1')
+    n = lib.sm3_gemm_packed_act_elems(T, 4 * C, 1, 128)
+    dh_mn = torch.empty((n,), device=b1.device, dtype=torch.int16)
+    a_mn = torch.empty((n,), device=b1.device, dtype=torch.int16)
+    mode = FFN_BWD_IMG if h is None else FFN_BWD_IMG_H
+    a = _ffn_args(T=T, C=C, chunk=chunk, mode=mode, a1=v_img if h is None else dz_img, a2=dz_img,
+                  wa1=w1_img if h is None else w2gt_img, wa2=w2gt_img, b1=b1, wb=w1t_img)
+    a.out = _p(out); a.dh_mn = dh_mn.data_ptr(); a.act_mn = a_mn.data_ptr(); a.db1 = _p(db1); a.h_in = _p(h)
     _lib.check(lib.sm3_ffn_fused(_ct.byref(a), _stream()), 'sm3_ffn_fused(bwd)')
-    return out
+    return out, dh_mn, a_mn
 
 
 def fused_cost(name, *a, **kw):
@@ -230,7 +251,12 @@ def fused_cost(name, *a, **kw):
     wbytes = 2 * 4.0 * 4 * Cc * Cc
     if name == 'ffn_fused_fwd':
         return 2 * unit, (3 + (1 if kw.get('want_aux') else 0) + (4 if kw.get('want_h') else 0)) * 4.0 * T * Cc + wbytes, (T, Cc, 'fwd')
-    return 2 * unit, 3 * 4.0 * T * Cc + 2 * wbytes, (T, Cc, 'bwd-dv')
+    if not kw.get('want_wgrad_images'):
+        return 2 * unit, 3 * 4.0 * T * Cc + 2 * wbytes, (T, Cc, 'bwd-dv')
+    # bytes per token x channel: dz image + dv (4 + 4), the v image (4, mode 2) or the saved fp32 h (16, mode 3), and the
+    # two [T,4C] hi|lo images (16 + 16)
+    h = kw.get('h') is not None
+    return 2 * unit, (8 + (16 if h else 4) + 32) * float(T * Cc) + 2 * wbytes, (T, Cc, 'bwd-img-h' if h else 'bwd-img')
 
 
 def act_pack(h, *, rows, width, mode, da=None, want_k=False, mn_tile=0, want_f32=False, colsum=None, live_tiles=None,
