@@ -326,6 +326,18 @@ int sm3_dropout(const float* x, float* out, int64_t n, float p, uint64_t seed, v
 /* Same mask function with the seed read from device memory (one uint64): a captured CUDA graph replays the launch while the
  * seed tensor is refreshed between replays, so every step still draws a new mask. */
 int sm3_dropout_dev(const float* x, float* out, int64_t n, float p, const uint64_t* seed_dev, void* stream);
+/* Mlp middle stage (Mlp.forward :307-311): a = drop(gelu(dwconv3x3(h) + bias)) on NHWC h [N,H,W,C], C % 32 == 0,
+ * weight_t = the 3x3 taps as [9][C].  Bit-identical to sm3_dwconv_fwd(ks 3) -> sm3_act_pack(GELU) -> sm3_dropout / sm3_mul
+ * with the same seed or mask; nothing but h is needed for the backward.  Dropout: mask != NULL multiplies by that
+ * pre-scaled keep mask; else p > 0 applies the sm3_dropout mask of `seed` (of *seed_dev when seed_dev != NULL, as
+ * sm3_dropout_dev); else none.
+ * sm3_mlp_mid_bwd: dh (bit-identical to the dgrad of that sequence) and dweight_t / dbias ACCUMULATED (+=) from da in one
+ * pass that recomputes gelu(dwconv(h)) from h. */
+int sm3_mlp_mid_fwd(const float* h, const float* weight_t, const float* bias, const float* mask, float* a, int32_t N,
+                    int32_t H, int32_t W, int32_t C, float p, uint64_t seed, const uint64_t* seed_dev, void* stream);
+int sm3_mlp_mid_bwd(const float* h, const float* weight_t, const float* bias, const float* da, const float* mask, float* dh,
+                    float* dweight_t, float* dbias, int32_t N, int32_t H, int32_t W, int32_t C, float p, uint64_t seed,
+                    const uint64_t* seed_dev, void* stream);
 int sm3_lsk_agg(const float* a1, const float* a2, float* agg, int32_t* amax, int64_t T, int32_t Ch, void* stream);
 int sm3_conv7_c2(const float* x, const float* w, const float* b, float* y, int32_t N, int32_t H, int32_t W, int32_t act,
                  void* stream);

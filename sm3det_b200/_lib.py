@@ -129,6 +129,10 @@ SIGNATURES = {
     'sm3_mul': [_P, _P, _P, _P, _I64, _P],
     'sm3_dropout': [_P, _P, _I64, _F32, C.c_uint64, _P],
     'sm3_dropout_dev': [_P, _P, _I64, _F32, _P, _P],
+    # h, weight_t, bias, mask, a, N, H, W, C, p, seed, seed_dev, stream
+    'sm3_mlp_mid_fwd': [_P, _P, _P, _P, _P, _I32, _I32, _I32, _I32, _F32, C.c_uint64, _P, _P],
+    # h, weight_t, bias, da, mask, dh, dweight_t, dbias, N, H, W, C, p, seed, seed_dev, stream
+    'sm3_mlp_mid_bwd': [_P, _P, _P, _P, _P, _P, _P, _P, _I32, _I32, _I32, _I32, _F32, C.c_uint64, _P, _P],
     'sm3_lsk_agg': [_P, _P, _P, _P, _I64, _I32, _P],
     'sm3_conv7_c2': [_P, _P, _P, _P, _I32, _I32, _I32, _I32, _P],
     'sm3_conv7_c2_wgrad': [_P, _P, _P, _P, _I32, _I32, _I32, _P],

@@ -217,6 +217,17 @@ int sm3_dropout(const float* x, float* out, int64_t n, float p, uint64_t seed, v
 int sm3_dropout_dev(const float* x, float* out, int64_t n, float p, const uint64_t* seed_dev, void* stream) {
   return dropout_dev(x, out, n, p, reinterpret_cast<const unsigned long long*>(seed_dev), S(stream));
 }
+int sm3_mlp_mid_fwd(const float* h, const float* weight_t, const float* bias, const float* mask, float* a, int32_t N,
+                    int32_t H, int32_t W, int32_t C, float p, uint64_t seed, const uint64_t* seed_dev, void* stream) {
+  return mlp_mid_fwd(h, weight_t, bias, mask, a, N, H, W, C, p, seed, reinterpret_cast<const unsigned long long*>(seed_dev),
+                     S(stream));
+}
+int sm3_mlp_mid_bwd(const float* h, const float* weight_t, const float* bias, const float* da, const float* mask, float* dh,
+                    float* dweight_t, float* dbias, int32_t N, int32_t H, int32_t W, int32_t C, float p, uint64_t seed,
+                    const uint64_t* seed_dev, void* stream) {
+  return mlp_mid_bwd(h, weight_t, bias, da, mask, dh, dweight_t, dbias, N, H, W, C, p, seed,
+                     reinterpret_cast<const unsigned long long*>(seed_dev), S(stream));
+}
 int sm3_lsk_agg(const float* a1, const float* a2, float* agg, int32_t* amax, int64_t T, int32_t Ch, void* stream) {
   return lsk_agg(a1, a2, agg, amax, T, Ch, S(stream));
 }

@@ -91,6 +91,19 @@ __device__ __forceinline__ float4 ldg_f4(const float* p) {
   return __ldg(reinterpret_cast<const float4*>(p));
 }
 
+// Counter-based dropout mask: element e of a tensor is kept when dropout_bits(seed, e) >= p * 2^32.  A pure function of
+// (seed, flat element index), so every kernel that applies or differentiates the same dropout draws the same mask.
+__device__ __forceinline__ uint32_t mix32(uint64_t z) {      // splitmix64 finaliser
+  z += 0x9E3779B97F4A7C15ull;
+  z = (z ^ (z >> 30)) * 0xBF58476D1CE4E5B9ull;
+  z = (z ^ (z >> 27)) * 0x94D049BB133111EBull;
+  return (uint32_t)((z ^ (z >> 31)) >> 32);
+}
+__device__ __forceinline__ uint32_t dropout_bits(uint64_t seed, long long e) {
+  const uint64_t base = seed ^ ((uint64_t)(e & ~3LL) * 0xD1342543DE82EF95ull);
+  return mix32(base + (uint64_t)(e & 3) * 0x632BE59BD9B4E019ull);
+}
+
 }  // namespace sm3
 
 // dispatch a kernel templated on V = C/32 (channels per lane)

@@ -163,6 +163,11 @@ int affine(const float* x1, const float* a1, const float* x2, const float* a2, c
 int mul(const float* a, const float* b, const float* add, float* out, long long n, cudaStream_t stream);
 int dropout(const float* x, float* out, long long n, float p, unsigned long long seed, cudaStream_t stream);
 int dropout_dev(const float* x, float* out, long long n, float p, const unsigned long long* seed_dev, cudaStream_t stream);
+int mlp_mid_fwd(const float* h, const float* wt, const float* bias, const float* mask, float* a, int N, int H, int W, int C,
+                float p, unsigned long long seed, const unsigned long long* seed_dev, cudaStream_t stream);
+int mlp_mid_bwd(const float* h, const float* wt, const float* bias, const float* da, const float* mask, float* dh, float* dwt,
+                float* dbias, int N, int H, int W, int C, float p, unsigned long long seed,
+                const unsigned long long* seed_dev, cudaStream_t stream);
 int lsk_agg(const float* a1, const float* a2, float* agg, int* amax, long long T, int Ch, cudaStream_t stream);
 int conv7_c2(const float* x, const float* w, const float* b, float* y, int N, int H, int W, int act, cudaStream_t stream);
 int conv7_c2_wgrad(const float* x, const float* dpre, float* dw, float* db, int N, int H, int W, cudaStream_t stream);

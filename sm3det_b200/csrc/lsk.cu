@@ -25,8 +25,8 @@ struct DwGeom {
 };
 
 template <int R, int TI>
-__device__ __forceinline__ void dwg_load_tile(float* xs, const float* __restrict__ x, int n, int h0, int w0, int c0, int H,
-                                              int W, int C) {
+__device__ __forceinline__ void dwg_issue_tile(float* xs, const float* __restrict__ x, int n, int h0, int w0, int c0, int H,
+                                               int W, int C) {
   for (int idx = threadIdx.x; idx < TI * TI * 8; idx += blockDim.x) {
     const int q = idx & 7, pix = idx >> 3;
     const int py = pix / TI, px = pix - py * TI;
@@ -39,8 +39,45 @@ __device__ __forceinline__ void dwg_load_tile(float* xs, const float* __restrict
       asm volatile("st.shared.v4.f32 [%0], {%1, %1, %1, %1};" ::"r"(dst), "f"(0.f) : "memory");
     }
   }
+}
+
+__device__ __forceinline__ void dwg_wait_tiles() {
   asm volatile("cp.async.commit_group;\n\tcp.async.wait_group 0;" ::: "memory");
   __syncthreads();
+}
+
+// stage the TI x TI x 32 input tile at (h0 - R, w0 - R) (zero outside the image) and wait for it
+template <int R, int TI>
+__device__ __forceinline__ void dwg_load_tile(float* xs, const float* __restrict__ x, int n, int h0, int w0, int c0, int H,
+                                              int W, int C) {
+  dwg_issue_tile<R, TI>(xs, x, n, h0, w0, c0, H, W, C);
+  dwg_wait_tiles();
+}
+
+// One output row of a tile for one channel pair: acc[o] = bias + sum over taps (i, j) in row-major order of
+// x[r + i*DIL][o + j*DIL] * wt[i*KS + j].  Shared by dwconv_tile_kernel and the fused Mlp middle stage, whose forward must
+// be bit-identical to this convolution followed by GELU and dropout.
+template <int KS, int DIL>
+__device__ __forceinline__ void dwg_tile_row(const float* xs, const float* __restrict__ wt, int C, int c, int r, int cp,
+                                             f32x2_t (&acc)[GT]) {
+  constexpr int TI = DwGeom<KS, DIL>::TI;
+  typedef f32x2_t f2;
+#pragma unroll 1
+  for (int i = 0; i < KS; ++i) {
+    f2 wv[KS];
+#pragma unroll
+    for (int j = 0; j < KS; ++j) wv[j] = __ldg(reinterpret_cast<const f2*>(wt + (i * KS + j) * C + c));
+    const f2* xr = reinterpret_cast<const f2*>(xs + ((r + i * DIL) * TI) * GCC) + cp;
+#pragma unroll
+    for (int cc = 0; cc < TI; ++cc) {
+      const f2 v = xr[cc * (GCC / 2)];
+#pragma unroll
+      for (int j = 0; j < KS; ++j) {
+        const int o = cc - j * DIL;
+        if (o >= 0 && o < GT) acc[o] = ffma2(v, wv[j], acc[o]);
+      }
+    }
+  }
 }
 
 // lane = (row selector l/16, channel pair l%16); ffma2 on channel pairs, as in stencil.cu's 7x7 kernel
@@ -65,22 +102,7 @@ __global__ void __launch_bounds__(256) dwconv_tile_kernel(const float* __restric
   f2 acc[GT];
 #pragma unroll
   for (int o = 0; o < GT; ++o) acc[o] = b2;
-#pragma unroll 1
-  for (int i = 0; i < KS; ++i) {
-    f2 wv[KS];
-#pragma unroll
-    for (int j = 0; j < KS; ++j) wv[j] = __ldg(reinterpret_cast<const f2*>(wt + (i * KS + j) * C + c));
-    const f2* xr = reinterpret_cast<const f2*>(xs + ((r + i * DIL) * TI) * GCC) + cp;
-#pragma unroll
-    for (int cc = 0; cc < TI; ++cc) {
-      const f2 v = xr[cc * (GCC / 2)];
-#pragma unroll
-      for (int j = 0; j < KS; ++j) {
-        const int o = cc - j * DIL;
-        if (o >= 0 && o < GT) acc[o] = ffma2(v, wv[j], acc[o]);
-      }
-    }
-  }
+  dwg_tile_row<KS, DIL>(xs, wt, C, c, r, cp, acc);
   const long long rowoff = (((long long)n * H + h) * W) * C + c;
 #pragma unroll
   for (int o = 0; o < GT; ++o) {
@@ -217,6 +239,201 @@ int dwconv_wgrad(const float* x, const float* dy, float* dwt, float* dbias, int 
 }
 
 // ------------------------------------------------------------------------------------------------
+// Mlp middle stage (lsk_moe.py Mlp.forward :307-311, lsknet.py :27-29):  a = drop(gelu(dwconv3x3(h) + b)).
+// Forward = the 3x3 tile kernel above with GELU and dropout in its epilogue: reads h, writes a, stores no u.
+// Backward = one pass per 16x16 tile: recompute u over the tile plus a one-pixel halo from h (two-pixel halo), form
+// du = drop(da) * gelu'(u) in shared memory, write dh with the flipped taps and accumulate dw / db from the same h and du.
+// Every value of a, u, du and dh is computed with the arithmetic, in the order, of dwconv_tile_kernel<3,1> -> act_pack ->
+// dropout_kernel (and back), so a and dh are bit-identical to that sequence; dw / db differ from dwconv_wgrad_tile_kernel
+// only in summation order.
+// Dropout: mask != null multiplies by the given (pre-scaled) mask; otherwise hashed != 0 applies the dropout_bits mask of
+// (seed, flat NHWC element index), the seed read from seed_dev when that is given (CUDA-graph replay); otherwise identity.
+struct MlpDrop {
+  const float* mask;
+  const unsigned long long* seed_dev;
+  unsigned long long seed;
+  uint32_t thresh;
+  float scale;
+  int hashed;
+};
+
+__device__ __forceinline__ float mlp_drop(const MlpDrop& d, uint64_t seed, float v, long long e) {
+  if (d.mask) return v * __ldg(d.mask + e);
+  if (d.hashed) return dropout_bits(seed, e) >= d.thresh ? v * d.scale : 0.f;
+  return v;
+}
+
+__global__ void __launch_bounds__(256) mlp_mid_fwd_kernel(const float* __restrict__ h, const float* __restrict__ wt,
+                                                         const float* __restrict__ bias, float* __restrict__ a, int H, int W,
+                                                         int C, int tiles_w, const MlpDrop drop) {
+  constexpr int R = DwGeom<3, 1>::R, TI = DwGeom<3, 1>::TI;
+  extern __shared__ float xs[];                           // [TI][TI][GCC]
+  const int tw = blockIdx.x % tiles_w, th = blockIdx.x / tiles_w;
+  const int cchunks = C / GCC;
+  const int n = blockIdx.y / cchunks, c0 = (blockIdx.y % cchunks) * GCC;
+  const int h0 = th * GT, w0 = tw * GT;
+  dwg_load_tile<R, TI>(xs, h, n, h0, w0, c0, H, W, C);
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const int cp = lane & 15, r = warp * 2 + (lane >> 4);
+  const int c = c0 + 2 * cp;
+  const int y = h0 + r;
+  if (y >= H) return;
+  const uint64_t seed = drop.seed_dev ? __ldg(drop.seed_dev) : drop.seed;
+  const f32x2_t b2 = __ldg(reinterpret_cast<const f32x2_t*>(bias + c));
+  f32x2_t acc[GT];
+#pragma unroll
+  for (int o = 0; o < GT; ++o) acc[o] = b2;
+  dwg_tile_row<3, 1>(xs, wt, C, c, r, cp, acc);
+  const long long rowoff = (((long long)n * H + y) * W) * C + c;
+#pragma unroll
+  for (int o = 0; o < GT; ++o) {
+    const int x = w0 + o;
+    if (x < W) {
+      const long long e = rowoff + (long long)x * C;
+      float2 v = make_float2(gelu_fast(__uint_as_float((uint32_t)acc[o])), gelu_fast(__uint_as_float((uint32_t)(acc[o] >> 32))));
+      v.x = mlp_drop(drop, seed, v.x, e);
+      v.y = mlp_drop(drop, seed, v.y, e + 1);
+      *reinterpret_cast<float2*>(a + e) = v;
+    }
+  }
+}
+
+constexpr int MM_TU = GT + 2;          // du / u tile edge (one-pixel halo)
+constexpr int MM_TH = GT + 4;          // h tile edge (two-pixel halo)
+
+// lane = channel; warps stride over the pixels of a tile.  Persistent blocks over the tiles of one 32-channel chunk keep
+// the 9 tap sums and the bias sum in registers, so the cross-block reduction is one atomic per (tap, channel) per block.
+__global__ void __launch_bounds__(256) mlp_mid_bwd_kernel(const float* __restrict__ h, const float* __restrict__ wt,
+                                                         const float* __restrict__ bias, const float* __restrict__ da,
+                                                         float* __restrict__ dh, float* __restrict__ dwt,
+                                                         float* __restrict__ dbias, int N, int H, int W, int C, int tiles_w,
+                                                         int tiles_h, int blocks_per_chunk, const MlpDrop drop) {
+  extern __shared__ float smem[];
+  float* hs = smem;                                // [MM_TH][MM_TH][GCC]
+  float* dus = smem + MM_TH * MM_TH * GCC;         // [MM_TU][MM_TU][GCC]: da, then du
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const int c0 = blockIdx.y * GCC, c = c0 + lane;
+  const uint64_t seed = drop.seed_dev ? __ldg(drop.seed_dev) : drop.seed;
+  float wv[9];
+#pragma unroll
+  for (int k = 0; k < 9; ++k) wv[k] = __ldg(wt + k * C + c);
+  const float b = __ldg(bias + c);
+  float gw[9], gb = 0.f;
+#pragma unroll
+  for (int k = 0; k < 9; ++k) gw[k] = 0.f;
+  const int tiles = N * tiles_h * tiles_w;
+  for (int t = blockIdx.x; t < tiles; t += blocks_per_chunk) {
+    const int n = t / (tiles_h * tiles_w), rem = t % (tiles_h * tiles_w);
+    const int h0 = (rem / tiles_w) * GT, w0 = (rem % tiles_w) * GT;
+    __syncthreads();                               // previous tile's hs / dus fully consumed
+    dwg_issue_tile<2, MM_TH>(hs, h, n, h0, w0, c0, H, W, C);
+    dwg_issue_tile<1, MM_TU>(dus, da, n, h0, w0, c0, H, W, C);     // da over the du tile; du overwrites it in place
+    dwg_wait_tiles();
+    for (int p = warp; p < MM_TU * MM_TU; p += 8) {
+      const int py = p / MM_TU, px = p - py * MM_TU;
+      const int y = h0 - 1 + py, x = w0 - 1 + px;
+      float du = 0.f;                              // zero outside the image: the padding of the dgrad stencil
+      if (y >= 0 && y < H && x >= 0 && x < W) {
+        float xv[9];
+        float u = b;
+#pragma unroll
+        for (int i = 0; i < 3; ++i)
+#pragma unroll
+          for (int j = 0; j < 3; ++j) {
+            xv[i * 3 + j] = hs[((py + i) * MM_TH + px + j) * GCC + lane];
+            u = fmaf(xv[i * 3 + j], wv[i * 3 + j], u);
+          }
+        const long long e = (((long long)n * H + y) * W + x) * C + c;
+        du = mlp_drop(drop, seed, dus[p * GCC + lane], e) * gelu_grad_fast(u);
+        if (py >= 1 && py <= GT && px >= 1 && px <= GT) {
+#pragma unroll
+          for (int k = 0; k < 9; ++k) gw[k] = fmaf(xv[k], du, gw[k]);
+          gb += du;
+        }
+      }
+      dus[p * GCC + lane] = du;
+    }
+    __syncthreads();
+    for (int p = warp; p < GT * GT; p += 8) {
+      const int oy = p / GT, ox = p - oy * GT;
+      const int y = h0 + oy, x = w0 + ox;
+      if (y >= H || x >= W) continue;
+      float acc = 0.f;
+#pragma unroll
+      for (int i = 0; i < 3; ++i)
+#pragma unroll
+        for (int j = 0; j < 3; ++j) acc = fmaf(dus[((oy + i) * MM_TU + ox + j) * GCC + lane], wv[8 - (i * 3 + j)], acc);
+      dh[(((long long)n * H + y) * W + x) * C + c] = acc;
+    }
+  }
+  __syncthreads();
+  float* red = smem;                               // [8][10][32]
+#pragma unroll
+  for (int k = 0; k < 9; ++k) red[(warp * 10 + k) * 32 + lane] = gw[k];
+  red[(warp * 10 + 9) * 32 + lane] = gb;
+  __syncthreads();
+  for (int idx = threadIdx.x; idx < 10 * 32; idx += blockDim.x) {
+    const int k = idx / 32, l = idx % 32;
+    float sum = 0.f;
+#pragma unroll
+    for (int w = 0; w < 8; ++w) sum += red[(w * 10 + k) * 32 + l];
+    if (k < 9) atomicAdd(dwt + k * C + c0 + l, sum);
+    else atomicAdd(dbias + c0 + l, sum);
+  }
+}
+
+static int mlp_drop_args(MlpDrop& d, const float* mask, float p, unsigned long long seed, const unsigned long long* seed_dev) {
+  SM3_REQUIRE(p >= 0.f && p < 1.f, SM3_ERR_INVALID_ARG, "mlp_mid: dropout p=%f outside [0, 1)", p);
+  d.mask = mask;
+  d.seed_dev = seed_dev;
+  d.seed = seed;
+  d.hashed = (!mask && p > 0.f) ? 1 : 0;
+  d.thresh = (uint32_t)((double)p * 4294967296.0);      // as sm3_dropout
+  d.scale = 1.0f / (1.0f - p);
+  return SM3_OK;
+}
+
+int mlp_mid_fwd(const float* h, const float* wt, const float* bias, const float* mask, float* a, int N, int H, int W, int C,
+                float p, unsigned long long seed, const unsigned long long* seed_dev, cudaStream_t stream) {
+  SM3_REQUIRE(h && wt && bias && a, SM3_ERR_INVALID_ARG, "mlp_mid_fwd: null argument");
+  SM3_REQUIRE(C % GCC == 0 && N > 0 && H > 0 && W > 0 && (long long)N * (C / GCC) < 65536, SM3_ERR_UNSUPPORTED_SHAPE,
+              "mlp_mid_fwd: C=%d must be a multiple of 32 (N*C/32 < 65536)", C);
+  MlpDrop d;
+  const int rc = mlp_drop_args(d, mask, p, seed, seed_dev);
+  if (rc != SM3_OK) return rc;
+  constexpr int TI = DwGeom<3, 1>::TI;
+  const int tiles_w = (W + GT - 1) / GT, tiles_h = (H + GT - 1) / GT;
+  const size_t smem = (size_t)TI * TI * GCC * sizeof(float);
+  cudaFuncSetAttribute(mlp_mid_fwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+  dim3 grid((unsigned)(tiles_w * tiles_h), (unsigned)(N * (C / GCC)));
+  mlp_mid_fwd_kernel<<<grid, 256, smem, stream>>>(h, wt, bias, a, H, W, C, tiles_w, d);
+  return check_launch("mlp_mid_fwd_kernel");
+}
+
+int mlp_mid_bwd(const float* h, const float* wt, const float* bias, const float* da, const float* mask, float* dh, float* dwt,
+                float* dbias, int N, int H, int W, int C, float p, unsigned long long seed,
+                const unsigned long long* seed_dev, cudaStream_t stream) {
+  SM3_REQUIRE(h && wt && bias && da && dh && dwt && dbias, SM3_ERR_INVALID_ARG, "mlp_mid_bwd: null argument");
+  SM3_REQUIRE(C % GCC == 0 && N > 0 && H > 0 && W > 0 && C / GCC < 65536, SM3_ERR_UNSUPPORTED_SHAPE,
+              "mlp_mid_bwd: C=%d must be a multiple of 32", C);
+  MlpDrop d;
+  const int rc = mlp_drop_args(d, mask, p, seed, seed_dev);
+  if (rc != SM3_OK) return rc;
+  const int tiles_w = (W + GT - 1) / GT, tiles_h = (H + GT - 1) / GT;
+  const int chunks = C / GCC;
+  const long long tiles = (long long)N * tiles_w * tiles_h;
+  SM3_REQUIRE(tiles < (1LL << 31), SM3_ERR_UNSUPPORTED_SHAPE, "mlp_mid_bwd: tensor too large");
+  int bpc = (num_sms() * 2 + chunks - 1) / chunks;        // ~2 resident blocks per SM over all channel chunks
+  if (bpc > tiles) bpc = (int)tiles;
+  if (bpc < 1) bpc = 1;
+  const size_t smem = (size_t)(MM_TH * MM_TH + MM_TU * MM_TU) * GCC * sizeof(float);
+  cudaFuncSetAttribute(mlp_mid_bwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+  dim3 grid((unsigned)bpc, (unsigned)chunks);
+  mlp_mid_bwd_kernel<<<grid, 256, smem, stream>>>(h, wt, bias, da, dh, dwt, dbias, N, H, W, C, tiles_w, tiles_h, bpc, d);
+  return check_launch("mlp_mid_bwd_kernel");
+}
+
+// ------------------------------------------------------------------------------------------------
 // Column statistics:  s1[c] += sum_r w * (x[r,c]-sh1[c]) ,  s2[c] += sum_r w * (x - sh1) * (y ? (y[r,c]-sh2[c])*sc2[c] : (x - sh1))
 //   BatchNorm forward  : y = null, sh1 = running_mean (shifted-data variance, one pass)
 //   BatchNorm backward : x = dy (sh1 = null), y = saved input, sh2 = mean, sc2 = rstd  ->  s1 = sum dy, s2 = sum dy*xhat
@@ -321,12 +538,7 @@ int mul(const float* a, const float* b, const float* add, float* out, long long 
 // Dropout with a counter-based mask (nn.Dropout of Mlp, lsk_moe.py:300,311,316): keep = hash(seed, element index) >= p,
 // out = x * keep / (1 - p).  The same call with dy as input is the backward (the mask is recomputed, never stored), so
 // dropout costs one read + one write instead of torch's rand / compare / scale / multiply passes and a saved mask.
-__device__ __forceinline__ uint32_t mix32(uint64_t z) {      // splitmix64 finaliser
-  z += 0x9E3779B97F4A7C15ull;
-  z = (z ^ (z >> 30)) * 0xBF58476D1CE4E5B9ull;
-  z = (z ^ (z >> 27)) * 0x94D049BB133111EBull;
-  return (uint32_t)((z ^ (z >> 31)) >> 32);
-}
+// (mask function: dropout_bits in common.cuh, shared with the fused Mlp middle stage below)
 __global__ void __launch_bounds__(256) dropout_kernel(const float* __restrict__ x, float* __restrict__ out, long long n4,
                                                      uint32_t thresh, float scale, uint64_t seed,
                                                      const unsigned long long* __restrict__ seed_dev) {
@@ -334,12 +546,11 @@ __global__ void __launch_bounds__(256) dropout_kernel(const float* __restrict__ 
   if (i >= n4) return;
   if (seed_dev) seed = __ldg(seed_dev);      // CUDA-graph replay: the seed lives in device memory and changes between replays
   const float4 v = ldg_f4(x + i * 4);
-  const uint64_t base = seed ^ ((uint64_t)i * 4ull * 0xD1342543DE82EF95ull);
   float4 o;
-  o.x = mix32(base) >= thresh ? v.x * scale : 0.f;
-  o.y = mix32(base + 0x632BE59BD9B4E019ull) >= thresh ? v.y * scale : 0.f;
-  o.z = mix32(base + 2ull * 0x632BE59BD9B4E019ull) >= thresh ? v.z * scale : 0.f;
-  o.w = mix32(base + 3ull * 0x632BE59BD9B4E019ull) >= thresh ? v.w * scale : 0.f;
+  o.x = dropout_bits(seed, i * 4) >= thresh ? v.x * scale : 0.f;
+  o.y = dropout_bits(seed, i * 4 + 1) >= thresh ? v.y * scale : 0.f;
+  o.z = dropout_bits(seed, i * 4 + 2) >= thresh ? v.z * scale : 0.f;
+  o.w = dropout_bits(seed, i * 4 + 3) >= thresh ? v.w * scale : 0.f;
   *reinterpret_cast<float4*>(out + i * 4) = o;
 }
 

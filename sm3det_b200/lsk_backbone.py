@@ -119,19 +119,25 @@ class Mlp(nn.Module):
         self.act = act_layer()
         self.drop = nn.Dropout(drop)
 
-    def _dropout(self, x):
+    def _drop_args(self, x):
+        """(p, seed, mask) of one nn.Dropout call on x: p = 0 is no dropout; a mask (injected by tests) replaces the seed."""
         p = self.drop.p
         if p == 0.0 or not self.training:
-            return x
+            return 0.0, 0, None
         masks = getattr(self, '_injected_drop_masks', None)
         if masks:                                   # tests inject the reference's masks
-            m = masks.pop(0).to(x.device, torch.float32).reshape(x.shape).contiguous()
-            return LF.MulFn.apply(x, m)
+            return p, 0, masks.pop(0).to(x.device, torch.float32).reshape(x.shape).contiguous()
         if torch.cuda.is_current_stream_capturing():
             seed = torch.randint(0, 2 ** 62, (1,), device=x.device)     # graph-safe: drawn on the device at every replay
         else:
             seed = int(torch.randint(0, 2 ** 62, (1,)).item())          # host RNG (torch.manual_seed reproducible), no device sync
-        return LF.DropoutFn.apply(x, p, seed)
+        return p, seed, None
+
+    def _dropout(self, x):
+        p, seed, mask = self._drop_args(x)
+        if mask is not None:
+            return LF.MulFn.apply(x, mask)
+        return x if p == 0.0 else LF.DropoutFn.apply(x, p, seed)
 
     def forward(self, x, ls, resid, row_scale, record=None):
         """x: NHWC BN output.  Returns (resid + row_scale * ls * mlp(x), loss or None)  (Block.forward :390-395)."""
@@ -142,9 +148,7 @@ class Mlp(nn.Module):
         else:
             x = _conv1x1(self.fc1, x)
         dw = self.dwconv.dwconv
-        x = LF.DWConvFn.apply(x, dw.weight, dw.bias, 3, 1)
-        x = LF.GeluFn.apply(x)
-        x = self._dropout(x)
+        x = LF.MlpMidFn.apply(x, dw.weight, dw.bias, *self._drop_args(x))      # dwconv -> act -> drop in one kernel
         final_drop = self.drop.p > 0.0 and self.training
         if self.MoE_cfg2 is not None:
             if final_drop:
@@ -462,3 +466,56 @@ class VAN_moe(LSKNet_moe):
 class VAN_moe_MultiInput(LSKNet_moe_MultiInput):
     """van_moe.py:590-814."""
     _spatial_unit = 'lka'
+
+
+def load_pretrained(module, checkpoint):
+    """mmcv load_checkpoint(module, checkpoint, strict=False): unwrap 'state_dict' / 'model', strip a leading 'module.',
+    load what matches by name and shape, warn about the rest.  No key remapping."""
+    import re
+    ckpt = torch.load(checkpoint, map_location='cpu')
+    sd = ckpt.get('state_dict', ckpt.get('model', ckpt)) if isinstance(ckpt, dict) else ckpt
+    sd = {re.sub(r'^module\.', '', k): v for k, v in sd.items()}
+    own = module.state_dict()
+    mismatched = [k for k, v in sd.items() if k in own and tuple(v.shape) != tuple(own[k].shape)]
+    res = module.load_state_dict({k: v for k, v in sd.items() if k not in mismatched}, strict=False)
+    if mismatched or res.missing_keys or res.unexpected_keys:
+        warnings.warn(f'{type(module).__name__}: checkpoint {checkpoint}: shape mismatch {mismatched}, missing keys '
+                      f'{res.missing_keys}, unexpected keys {res.unexpected_keys}')
+    return res
+
+
+@ROTATED_BACKBONES.register_module()
+class LSKNet(LSKNet_moe):
+    """Dense single-dataset LSKNet (lsknet.py:128-221): the LSKNet_moe module tree with no expert layer, so the
+    state_dict keys are the reference's.  forward(x) returns a list of the 4 NCHW maps; a Pretrained init_cfg loads the
+    checkpoint as it is (no expert up-cycling)."""
+
+    def __init__(self, img_size=224, in_chans=3, embed_dims=[64, 128, 256, 512], mlp_ratios=[8, 8, 4, 4], drop_rate=0.,
+                 drop_path_rate=0., norm_layer=partial(nn.LayerNorm, eps=1e-6), depths=[3, 4, 6, 3], num_stages=4,
+                 pretrained=None, init_cfg=None, norm_cfg=None):
+        super().__init__(MoE_Block_inds_fc1=[[]] * num_stages, MoE_Block_inds_fc2=[[]] * num_stages, img_size=img_size,
+                         in_chans=in_chans, embed_dims=embed_dims, mlp_ratios=mlp_ratios, drop_rate=drop_rate,
+                         drop_path_rate=drop_path_rate, norm_layer=norm_layer, depths=depths, num_stages=num_stages,
+                         pretrained=pretrained, init_cfg=init_cfg, norm_cfg=norm_cfg)
+
+    def init_weights(self):
+        cfg = self.init_cfg
+        if isinstance(cfg, dict) and cfg.get('type') == 'Pretrained' and cfg.get('checkpoint'):
+            load_pretrained(self, cfg['checkpoint'])
+            return
+        super().init_weights()
+
+    def forward(self, x):
+        return list(super().forward(x))
+
+
+@ROTATED_BACKBONES.register_module()
+class VAN(LSKNet):
+    """Dense single-dataset VAN (van.py:116-211): LSKNet with the LKA gating unit; forward(x, datasets) concatenates a
+    list input along the batch."""
+    _spatial_unit = 'lka'
+
+    def forward(self, x, datasets=['single']):
+        if isinstance(x, list):
+            x = torch.cat(x, dim=0)
+        return super().forward(x)

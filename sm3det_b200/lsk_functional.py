@@ -4,8 +4,9 @@ Each Function only sequences C-ABI kernel calls (sm3det_b200.ops); activations s
 replaces in the reference (mmrotate/models/backbones/lsk_moe.py):
   BatchNormFn    nn.BatchNorm2d / SyncBatchNorm built by build_norm_layer        :369-374, :407-410, :692-695
   LinearFn       every 1x1 nn.Conv2d (proj_1/2, conv1/2, conv, fc1/fc2) (+GELU)  :324-327, :351-354, :293-298
-  DWConvFn       depthwise 5x5, 7x7 dilation 3, 3x3                              :322-323, :583
-  GeluFn         Mlp.act                                                         :310
+  DWConvFn       depthwise 5x5, 7x7 dilation 3                                   :322-323
+  GeluFn         GELU (tests compare MlpMidFn against DWConvFn -> GeluFn -> DropoutFn)
+  MlpMidFn       Mlp.dwconv (3x3) + Mlp.act + the first Mlp.drop, one kernel     :583, :309-311
   LSKSelectFn    mean/max -> conv_squeeze -> sigmoid -> weighted sum             :335-341
   MulFn          x * attn, dropout masks                                         :343, :311, :316
   AxpyFn         layer-scale * branch + shortcut                                 :362, :388-395
@@ -238,6 +239,31 @@ class DropoutFn(Function):
     @staticmethod
     def backward(ctx, d):
         return ops.dropout(d.contiguous(), ctx.p, ctx.seed), None, None
+
+
+@ops.captures_precision
+class MlpMidFn(Function):
+    """Mlp middle stage a = dropout(gelu(dwconv3x3(h) + b)) in one kernel each way; bit-identical (forward and dh) to
+    DWConvFn(3, 1) -> GeluFn -> DropoutFn (or MulFn with ``mask``).  Saves only h.  p = 0 without a mask: no dropout."""
+
+    @staticmethod
+    def forward(ctx, h, w, b, p, seed, mask):
+        h = h.contiguous()
+        mask = None if mask is None else mask.contiguous()
+        a = ops.mlp_mid_fwd(h, _taps(w), b, p=p, seed=seed, mask=mask)
+        if any(ctx.needs_input_grad):
+            ctx.save_for_backward(h, w, b, mask)
+            ctx.p, ctx.seed = p, seed
+        return a
+
+    @staticmethod
+    def backward(ctx, da):
+        h, w, b, mask = ctx.saved_tensors
+        C = h.shape[-1]
+        dwt = torch.zeros((9, C), device=h.device, dtype=torch.float32)
+        db = torch.zeros((C,), device=h.device, dtype=torch.float32)
+        dh = ops.mlp_mid_bwd(h, _taps(w), b, da.contiguous(), dwt, db, p=ctx.p, seed=ctx.seed, mask=mask)
+        return dh, dwt.t().reshape(w.shape).contiguous(), db, None, None, None
 
 
 @ops.captures_precision

@@ -646,6 +646,37 @@ def dropout(x, p, seed):
     return out
 
 
+def _drop_seed(seed):
+    """(host seed, device seed pointer) of a dropout seed: a python int, or an int64 device tensor [1]."""
+    if torch.is_tensor(seed):
+        assert seed.is_cuda and seed.dtype == torch.int64 and seed.numel() == 1
+        return 0, seed.data_ptr()
+    return int(seed), None
+
+
+def mlp_mid_fwd(h, wt, bias, *, p=0.0, seed=0, mask=None):
+    """a = dropout(gelu(dwconv3x3(h) + bias)) on NHWC h (sm3_mlp_mid_fwd); wt = taps [9, C].  ``mask`` (pre-scaled keep
+    mask, h's shape) replaces the hashed mask of ``seed``; p = 0 without a mask is no dropout."""
+    lib = _lib.load()
+    N, H, W, Cc = h.shape
+    out = torch.empty_like(h)
+    s, sdev = _drop_seed(seed)
+    _lib.check(lib.sm3_mlp_mid_fwd(_p(h), _p(wt), _p(bias), _p(mask), _p(out), N, H, W, Cc, float(p), s, sdev, _stream()),
+               'sm3_mlp_mid_fwd')
+    return out
+
+
+def mlp_mid_bwd(h, wt, bias, da, dwt, dbias, *, p=0.0, seed=0, mask=None):
+    """dh of mlp_mid_fwd; dwt [9, C] and dbias [C] are accumulated."""
+    lib = _lib.load()
+    N, H, W, Cc = h.shape
+    dh = torch.empty_like(h)
+    s, sdev = _drop_seed(seed)
+    _lib.check(lib.sm3_mlp_mid_bwd(_p(h), _p(wt), _p(bias), _p(da), _p(mask), _p(dh), _p(dwt), _p(dbias), N, H, W, Cc,
+                                   float(p), s, sdev, _stream()), 'sm3_mlp_mid_bwd')
+    return dh
+
+
 def lsk_agg(a1, a2, *, T, Ch, want_idx=True):
     lib = _lib.load()
     agg = torch.empty((T, 2), device=a1.device, dtype=torch.float32)
