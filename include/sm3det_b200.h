@@ -362,6 +362,19 @@ int sm3_upsample_add_bwd(const float* d, float* db, int32_t N, int32_t H, int32_
                          void* stream);
 int sm3_transpose_batched(const float* in, float* out, int32_t B, int32_t R, int32_t Cc, void* stream);
 
+/* ---- mmdet FPN (add_extra_convs=False): the top level and its max-pool extra levels --------------------------------
+ * sm3_fpn_export_pool: in = P_top [N,H,W,C] (NHWC); outs = HOST array of L+1 device pointers, 1 <= L <=
+ * SM3_FPN_MAX_POOL_LEVELS: outs[0] = P_top [N,C,H,W], outs[k] = F.max_pool2d(level k-1, 1, stride=2) [N,C,H_k,W_k] with
+ * H_k = ceil(H_{k-1}/2), i.e. level k[y,x] = P_top[y<<k, x<<k].  One launch.
+ * sm3_fpn_export_pool_bwd: douts = HOST array of the L+1 upstream gradients (same shapes as outs);
+ * din[n,y,x,c] = douts[0][n,c,y,x] + sum_{k=1..L} [2^k | y, 2^k | x] douts[k][n,c,y>>k,x>>k], summed in that order by one
+ * thread per element (deterministic). */
+#define SM3_FPN_MAX_POOL_LEVELS 8
+int sm3_fpn_export_pool(const float* in, float* const* outs, int32_t N, int32_t H, int32_t W, int32_t C, int32_t L,
+                        void* stream);
+int sm3_fpn_export_pool_bwd(const float* const* douts, float* din, int32_t N, int32_t H, int32_t W, int32_t C, int32_t L,
+                            void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -121,6 +121,9 @@ SIGNATURES = {
     'sm3_upsample_add': [_P, _P, _P, _I32, _I32, _I32, _I32, _I32, _I32, _P],
     'sm3_upsample_add_bwd': [_P, _P, _I32, _I32, _I32, _I32, _I32, _I32, _P],
     'sm3_transpose_batched': [_P, _P, _I32, _I32, _I32, _P],
+    # in / din, host array of L+1 level pointers, N, H, W, C, L, stream
+    'sm3_fpn_export_pool': [_P, _P, _I32, _I32, _I32, _I32, _I32, _P],
+    'sm3_fpn_export_pool_bwd': [_P, _P, _I32, _I32, _I32, _I32, _I32, _P],
     # LSKNet-MoE
     'sm3_dwconv_fwd': [_P, _P, _P, _P, _P, _I32, _I32, _I32, _I32, _I32, _I32, _P],
     'sm3_dwconv_wgrad': [_P, _P, _P, _P, _I32, _I32, _I32, _I32, _I32, _I32, _P],

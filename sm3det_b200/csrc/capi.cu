@@ -279,5 +279,13 @@ int sm3_upsample_add_bwd(const float* d, float* db, int32_t N, int32_t H, int32_
 int sm3_transpose_batched(const float* in, float* out, int32_t B, int32_t R, int32_t Cc, void* stream) {
   return transpose_batched(in, out, B, R, Cc, S(stream));
 }
+int sm3_fpn_export_pool(const float* in, float* const* outs, int32_t N, int32_t H, int32_t W, int32_t C, int32_t L,
+                        void* stream) {
+  return fpn_export_pool(in, outs, N, H, W, C, L, S(stream));
+}
+int sm3_fpn_export_pool_bwd(const float* const* douts, float* din, int32_t N, int32_t H, int32_t W, int32_t C, int32_t L,
+                            void* stream) {
+  return fpn_export_pool_bwd(douts, din, N, H, W, C, L, S(stream));
+}
 
 }  // extern "C"

@@ -185,5 +185,7 @@ int col2im(const float* dcol, float* dx, int N, int H, int W, int Cin, int ks, i
 int upsample_add(const float* a, const float* b, float* out, int N, int H, int W, int h, int w, int C, cudaStream_t stream);
 int upsample_add_bwd(const float* d, float* db, int N, int H, int W, int h, int w, int C, cudaStream_t stream);
 int transpose_batched(const float* in, float* out, int B, int R, int Cc, cudaStream_t stream);
+int fpn_export_pool(const float* in, float* const* outs, int N, int H, int W, int C, int L, cudaStream_t stream);
+int fpn_export_pool_bwd(const float* const* douts, float* din, int N, int H, int W, int C, int L, cudaStream_t stream);
 
 }  // namespace sm3

@@ -770,3 +770,36 @@ def transpose_batched(x, B, R, Cc, out_shape):
     out = torch.empty(out_shape, device=x.device, dtype=torch.float32)
     _lib.check(lib.sm3_transpose_batched(_p(x), _p(out), B, R, Cc, _stream()), 'sm3_transpose_batched')
     return out
+
+
+def fpn_pool_shapes(N, C, H, W, L):
+    """NCHW shapes of P_top and its L max_pool2d(., 1, stride=2) levels: each level is ceil(H/2) x ceil(W/2) of the last."""
+    shapes = [(N, C, H, W)]
+    for _ in range(L):
+        H, W = (H + 1) // 2, (W + 1) // 2
+        shapes.append((N, C, H, W))
+    return shapes
+
+
+def _ptr_array(ts):
+    """Host array of device pointers (the kernel receives them by value, so the array may die after the call)."""
+    return (C.c_void_p * len(ts))(*[_p(t) for t in ts])
+
+
+def fpn_export_pool(x, L):
+    """x = P_top [N,H,W,C] (NHWC) -> (P_top NCHW, pool level 1, ..., pool level L), all NCHW."""
+    lib = _lib.load()
+    N, H, W, Cc = x.shape
+    outs = [torch.empty(s, device=x.device, dtype=torch.float32) for s in fpn_pool_shapes(N, Cc, H, W, L)]
+    _lib.check(lib.sm3_fpn_export_pool(_p(x), _ptr_array(outs), N, H, W, Cc, L, _stream()), 'sm3_fpn_export_pool')
+    return tuple(outs)
+
+
+def fpn_export_pool_bwd(ds):
+    """ds = the L+1 NCHW gradients of fpn_export_pool's outputs -> the NHWC gradient of its input."""
+    lib = _lib.load()
+    N, Cc, H, W = ds[0].shape
+    din = torch.empty((N, H, W, Cc), device=ds[0].device, dtype=torch.float32)
+    _lib.check(lib.sm3_fpn_export_pool_bwd(_ptr_array(ds), _p(din), N, H, W, Cc, len(ds) - 1, _stream()),
+               'sm3_fpn_export_pool_bwd')
+    return din
