@@ -6,7 +6,7 @@ NVFLAGS := $(ARCH) -O3 -std=c++17 -lineinfo -Xcompiler -fPIC -Xcompiler -Wall -I
 SRC := sm3det_b200/csrc
 OBJ := build/obj
 LIB := sm3det_b200/lib/libsm3det_b200.so
-SRCS := common.cu gemm_tc.cu ffn_fused.cu norm.cu stencil.cu front.cu moe.cu reduce.cu act.cu lsk.cu neck.cu capi.cu
+SRCS := common.cu gemm_tc.cu ffn_fused.cu norm.cu stencil.cu front.cu moe.cu reduce.cu act.cu lsk.cu neck.cu rpn_head.cu capi.cu
 OBJS := $(SRCS:%.cu=$(OBJ)/%.o)
 
 all: $(LIB)

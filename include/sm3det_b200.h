@@ -375,6 +375,33 @@ int sm3_fpn_export_pool(const float* in, float* const* outs, int32_t N, int32_t 
 int sm3_fpn_export_pool_bwd(const float* const* douts, float* din, int32_t N, int32_t H, int32_t W, int32_t C, int32_t L,
                             void* stream);
 
+/* ---- OrientedRPNHead (mmrotate/models/dense_heads/oriented_rpn_head.py:18-24): rpn_conv 3x3 -> ReLU -> rpn_cls / rpn_reg 1x1
+ * Levels: `shapes` = HOST array [L][3] of (N, H, W), 1 <= L <= SM3_RPN_MAX_LEVELS; the level pointer arguments are HOST arrays
+ * of L device pointers.  Row space: level l owns rows [R_l, R_l + ceil128(N H W)) with R_0 = 0, position (n, y, x) at row
+ * R_l + (n H + y) W + x; sm3_rpn_head_rows gives the total (the padding rows are never read as positions).
+ * sm3_rpn_head_fwd: cls[l] = [N,ncls,H,W], reg[l] = [N,nreg,H,W] (NCHW) from x[l] = [N,Cin,H,W]; one launch for all levels.
+ *   wconv_img: sm3_gemm_pack_b_tile(tile 256) of the conv weight as [256][9 * Cin] with k = (ky * 3 + kx) * Cin + c;
+ *   whead_img: sm3_gemm_pack_b_tile(tile 32) of [rpn_cls; rpn_reg] as [32][256], zero rows past ncls + nreg.
+ *   h_out (optional, [rows][256]): the ReLU output the backward reads.  Cin % 32 == 0, 32 <= Cin <= 256, ncls + nreg <= 32.
+ * sm3_rpn_head_mid_bwd: dpre[row, j] = (sum_o [dcls|dreg][row, o] Wh[o, j]) * [h[row, j] > 0] for every row (0 on padding
+ *   rows, fixed summation order); dwhead [ncls+nreg][256], dbhead, dbconv [256] are ACCUMULATED (+=, atomics).
+ * sm3_rpn_head_dx: dx[l] = [N,Cin,H,W] (NCHW, overwritten) = the 3x3 conv of dpre with wdx_img = sm3_gemm_pack_b_tile(tile 256)
+ *   of the flipped, transposed weight [Cin rows padded to 256][9 * 256], row c, k = (ky * 3 + kx) * 256 + o holding
+ *   W[o, c, 2 - ky, 2 - kx].
+ * sm3_rpn_head_tap_index: idx[tap][row] (int32 [9][rows]) = row of the neighbour (y + ky - 1, x + kx - 1), -1 outside the map
+ *   and on padding rows: the reduction-index gather of the per-tap weight-gradient GEMMs (sm3_gemm b_k_index). */
+#define SM3_RPN_MAX_LEVELS 8
+int64_t sm3_rpn_head_rows(const int32_t* shapes, int32_t L);
+int sm3_rpn_head_fwd(const float* const* x, float* const* cls, float* const* reg, const int32_t* shapes, int32_t L, int32_t Cin,
+                     const uint16_t* wconv_img, const float* bconv, const uint16_t* whead_img, const float* bhead, int32_t ncls,
+                     int32_t nreg, float* h_out, int32_t mma_passes, void* stream);
+int sm3_rpn_head_mid_bwd(const float* h, const float* const* dcls, const float* const* dreg, const int32_t* shapes, int32_t L,
+                         const float* whead, int32_t ncls, int32_t nreg, float* dpre, float* dwhead, float* dbhead, float* dbconv,
+                         void* stream);
+int sm3_rpn_head_dx(const float* dpre, float* const* dx, const int32_t* shapes, int32_t L, int32_t Cin, const uint16_t* wdx_img,
+                    int32_t mma_passes, void* stream);
+int sm3_rpn_head_tap_index(const int32_t* shapes, int32_t L, int32_t* idx, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

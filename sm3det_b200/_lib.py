@@ -124,6 +124,15 @@ SIGNATURES = {
     # in / din, host array of L+1 level pointers, N, H, W, C, L, stream
     'sm3_fpn_export_pool': [_P, _P, _I32, _I32, _I32, _I32, _I32, _P],
     'sm3_fpn_export_pool_bwd': [_P, _P, _I32, _I32, _I32, _I32, _I32, _P],
+    # OrientedRPNHead: host shape array [L][3] = (N, H, W), host arrays of level pointers
+    'sm3_rpn_head_rows': [_P, _I32],
+    # x, cls, reg, shapes, L, Cin, wconv_img, bconv, whead_img, bhead, ncls, nreg, h_out, mma_passes, stream
+    'sm3_rpn_head_fwd': [_P, _P, _P, _P, _I32, _I32, _P, _P, _P, _P, _I32, _I32, _P, _I32, _P],
+    # h, dcls, dreg, shapes, L, whead, ncls, nreg, dpre, dwhead, dbhead, dbconv, stream
+    'sm3_rpn_head_mid_bwd': [_P, _P, _P, _P, _I32, _P, _I32, _I32, _P, _P, _P, _P, _P],
+    # dpre, dx, shapes, L, Cin, wdx_img, mma_passes, stream
+    'sm3_rpn_head_dx': [_P, _P, _P, _I32, _I32, _P, _I32, _P],
+    'sm3_rpn_head_tap_index': [_P, _I32, _P, _P],
     # LSKNet-MoE
     'sm3_dwconv_fwd': [_P, _P, _P, _P, _P, _I32, _I32, _I32, _I32, _I32, _I32, _P],
     'sm3_dwconv_wgrad': [_P, _P, _P, _P, _I32, _I32, _I32, _I32, _I32, _I32, _P],
@@ -145,7 +154,7 @@ SIGNATURES = {
     'sm3_im2col': [_P, _P, _I32, _I32, _I32, _I32, _I32, _I32, _I32, _I32, _I32, _P],
     'sm3_col2im': [_P, _P, _I32, _I32, _I32, _I32, _I32, _I32, _I32, _I32, _I32, _P],
 }
-_RESTYPES = {'sm3_last_error': C.c_char_p, 'sm3_gemm_packed_elems': C.c_int64, 'sm3_gemm_packed_act_elems': C.c_int64,
+_RESTYPES = {'sm3_last_error': C.c_char_p, 'sm3_gemm_packed_elems': C.c_int64, 'sm3_gemm_packed_act_elems': C.c_int64, 'sm3_rpn_head_rows': C.c_int64,
              'sm3_gemm_workspace_bytes': C.c_size_t, 'sm3_ffn_fused_workspace_bytes': C.c_size_t,
              'sm3_moe_router_workspace_bytes': C.c_size_t, 'sm3_moe_plan_workspace_bytes': C.c_size_t}
 

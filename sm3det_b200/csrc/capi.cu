@@ -288,4 +288,23 @@ int sm3_fpn_export_pool_bwd(const float* const* douts, float* din, int32_t N, in
   return fpn_export_pool_bwd(douts, din, N, H, W, C, L, S(stream));
 }
 
+int64_t sm3_rpn_head_rows(const int32_t* shapes, int32_t L) { return rpn::rows(shapes, L); }
+int sm3_rpn_head_fwd(const float* const* x, float* const* cls, float* const* reg, const int32_t* shapes, int32_t L, int32_t Cin,
+                     const uint16_t* wconv_img, const float* bconv, const uint16_t* whead_img, const float* bhead, int32_t ncls,
+                     int32_t nreg, float* h_out, int32_t mma_passes, void* stream) {
+  return rpn::conv_fwd(x, cls, reg, shapes, L, Cin, wconv_img, bconv, whead_img, bhead, ncls, nreg, h_out, mma_passes, S(stream));
+}
+int sm3_rpn_head_mid_bwd(const float* h, const float* const* dcls, const float* const* dreg, const int32_t* shapes, int32_t L,
+                         const float* whead, int32_t ncls, int32_t nreg, float* dpre, float* dwhead, float* dbhead, float* dbconv,
+                         void* stream) {
+  return rpn::mid_bwd(h, dcls, dreg, shapes, L, whead, ncls, nreg, dpre, dwhead, dbhead, dbconv, S(stream));
+}
+int sm3_rpn_head_dx(const float* dpre, float* const* dx, const int32_t* shapes, int32_t L, int32_t Cin, const uint16_t* wdx_img,
+                    int32_t mma_passes, void* stream) {
+  return rpn::conv_dx(dpre, dx, shapes, L, Cin, wdx_img, mma_passes, S(stream));
+}
+int sm3_rpn_head_tap_index(const int32_t* shapes, int32_t L, int32_t* idx, void* stream) {
+  return rpn::tap_index(shapes, L, idx, S(stream));
+}
+
 }  // extern "C"

@@ -188,4 +188,18 @@ int transpose_batched(const float* in, float* out, int B, int R, int Cc, cudaStr
 int fpn_export_pool(const float* in, float* const* outs, int N, int H, int W, int C, int L, cudaStream_t stream);
 int fpn_export_pool_bwd(const float* const* douts, float* din, int N, int H, int W, int C, int L, cudaStream_t stream);
 
+
+// rpn_head.cu ------------------------------------------------------------------------------------
+namespace rpn {
+long long rows(const int* shapes, int L);
+int conv_fwd(const float* const* x, float* const* cls, float* const* reg, const int* shapes, int L, int Cin,
+             const uint16_t* wimg, const float* bconv, const uint16_t* himg, const float* bhead, int ncls, int nreg,
+             float* h_out, int passes, cudaStream_t stream);
+int mid_bwd(const float* h, const float* const* dcls, const float* const* dreg, const int* shapes, int L, const float* whead,
+            int ncls, int nreg, float* dpre, float* dwhead, float* dbhead, float* dbconv, cudaStream_t stream);
+int conv_dx(const float* dpre, float* const* dx, const int* shapes, int L, int Cin, const uint16_t* wimg, int passes,
+            cudaStream_t stream);
+int tap_index(const int* shapes, int L, int* idx, cudaStream_t stream);
+}  // namespace rpn
+
 }  // namespace sm3

@@ -803,3 +803,76 @@ def fpn_export_pool_bwd(ds):
     _lib.check(lib.sm3_fpn_export_pool_bwd(_ptr_array(ds), _p(din), N, H, W, Cc, len(ds) - 1, _stream()),
                'sm3_fpn_export_pool_bwd')
     return din
+
+
+# ---- OrientedRPNHead ---------------------------------------------------------------------------------------------------
+RPN_MAX_LEVELS = 8
+
+
+def _shape_array(shapes):
+    """Host int32 array [L][3] of the levels' (N, H, W)."""
+    flat = [int(v) for s in shapes for v in s]
+    return (C.c_int32 * len(flat))(*flat)
+
+
+def rpn_head_rows(shapes) -> int:
+    """Rows of the head's row space: every level padded to whole 128-row tiles."""
+    r = _lib.load().sm3_rpn_head_rows(_shape_array(shapes), len(shapes))
+    if r < 0:
+        _lib.check(int(r), 'sm3_rpn_head_rows')
+    return int(r)
+
+
+def rpn_head_fwd(xs, wconv_img, bconv, whead_img, bhead, *, ncls, nreg, want_h=False):
+    """xs = NCHW level maps -> (cls list, reg list, h [rows, 256] or None), one launch over every level."""
+    lib = _lib.load()
+    shapes = [(x.shape[0], x.shape[2], x.shape[3]) for x in xs]
+    dev = xs[0].device
+    cls = [torch.empty((n, ncls, h, w), device=dev, dtype=torch.float32) for n, h, w in shapes]
+    reg = [torch.empty((n, nreg, h, w), device=dev, dtype=torch.float32) for n, h, w in shapes]
+    hbuf = torch.empty((rpn_head_rows(shapes), 256), device=dev, dtype=torch.float32) if want_h else None
+    _lib.check(lib.sm3_rpn_head_fwd(_ptr_array(xs), _ptr_array(cls), _ptr_array(reg), _shape_array(shapes), len(xs),
+                                    xs[0].shape[1], _p(wconv_img, torch.int16), _p(bconv), _p(whead_img, torch.int16), _p(bhead),
+                                    ncls, nreg, _p(hbuf), current_passes(), _stream()), 'sm3_rpn_head_fwd')
+    return cls, reg, hbuf
+
+
+def rpn_head_mid_bwd(h, dcls, dreg, whead, dwhead, dbhead, dbconv, *, ncls, nreg):
+    """dpre [rows, 256] = ([dcls|dreg] @ whead) * (h > 0); dwhead / dbhead / dbconv accumulated (+=)."""
+    lib = _lib.load()
+    shapes = [(d.shape[0], d.shape[2], d.shape[3]) for d in dcls]
+    dpre = torch.empty_like(h)
+    _lib.check(lib.sm3_rpn_head_mid_bwd(_p(h), _ptr_array(dcls), _ptr_array(dreg), _shape_array(shapes), len(shapes), _p(whead),
+                                        ncls, nreg, _p(dpre), _p(dwhead), _p(dbhead), _p(dbconv), _stream()),
+               'sm3_rpn_head_mid_bwd')
+    return dpre
+
+
+def rpn_head_dx(dpre, shapes, Cin, wdx_img):
+    """dx per level (NCHW [N, Cin, H, W]) = the 3x3 conv of dpre with the flipped, transposed weight image."""
+    lib = _lib.load()
+    dx = [torch.empty((n, Cin, h, w), device=dpre.device, dtype=torch.float32) for n, h, w in shapes]
+    _lib.check(lib.sm3_rpn_head_dx(_p(dpre), _ptr_array(dx), _shape_array(shapes), len(shapes), Cin, _p(wdx_img, torch.int16),
+                                   current_passes(), _stream()), 'sm3_rpn_head_dx')
+    return dx
+
+
+def rpn_head_tap_index(shapes, device):
+    """int32 [9, rows]: the row each position reads for tap (ky, kx), -1 outside the map and on padding rows."""
+    lib = _lib.load()
+    idx = torch.empty((9, rpn_head_rows(shapes)), device=device, dtype=torch.int32)
+    _lib.check(lib.sm3_rpn_head_tap_index(_shape_array(shapes), len(shapes), _pi(idx), _stream()), 'sm3_rpn_head_tap_index')
+    return idx
+
+
+def rpn_head_nhwc_rows(xs, rows):
+    """The NCHW level maps as NHWC rows [rows, C] in the head's row space (padding rows left unwritten: never gathered)."""
+    lib = _lib.load()
+    Cc = xs[0].shape[1]
+    out = torch.empty((rows, Cc), device=xs[0].device, dtype=torch.float32)
+    r0 = 0
+    for x in xs:
+        N, _, H, W = x.shape
+        _lib.check(lib.sm3_transpose_batched(_p(x), out[r0:].data_ptr(), N, Cc, H * W, _stream()), 'sm3_transpose_batched')
+        r0 += -(-N * H * W // 128) * 128
+    return out
